@@ -218,6 +218,19 @@ int frcnn_detect_post(const float* cls_prob_dev, const float* pred_boxes_dev, co
                       int num_classes, float score_thresh, float nms_thresh, unsigned flags,
                       int max_per_image, int max_det, float* det_dev, int* ndet_dev, int record_stride, int* keep_dev,
                       int* keep_cnt_dev, float* keep_score_dev, void* workspace_dev, size_t workspace_bytes, void* stream);
+/* per-detection head features, run after frcnn_detect_post on the same keep_dev / keep_cnt_dev: slot k of image b is record
+ * row k of that image (classes ascending, slot = prefix(keep_cnt)[c] + j, slot < max_det).  fc7_dev [batch*r, feat_dim] is the
+ * head output the class / box FC read (feat_dim % 4 == 0, 16-byte aligned).  roi_out_dev int32 [batch, max_det] = RoI index
+ * within the image, -1 past the image's detection count; feat_out_dev [batch, max_det, feat_dim] = fc7 row of that RoI, zeros
+ * past the count. */
+int frcnn_detect_features(const int* keep_dev, const int* keep_cnt_dev, const float* fc7_dev, int r, int batch, int num_classes,
+                          int feat_dim, int max_det, float* feat_out_dev, int* roi_out_dev, void* stream);
+/* caller boxes -> RoI rows (the Fast R-CNN mode: TEST.HAS_RPN = False).  boxes_dev [batch, cap, 4] fp32 (x1,y1,x2,y2) in
+ * ORIGINAL-image pixels; counts_dev int32 [batch]; im_meta_dev [batch, 3] as for frcnn_bbox_decode.  rois_dev [batch*cap, 5] =
+ * (b, x1*s, y1*s, x2*s, y2*s), one fp32 multiply by im_meta's scale per coordinate, zeros past the count; num_rois_dev int32
+ * [batch] = min(count, cap).  No clipping: crop_and_resize samples outside the feature map as 0. */
+int frcnn_boxes_to_rois(const float* boxes_dev, const int* counts_dev, const float* im_meta_dev, int batch, int cap,
+                        float* rois_dev, int* num_rois_dev, void* stream);
 
 #ifdef __cplusplus
 }

@@ -65,6 +65,8 @@ SIGNATURES = {
     "frcnn_bbox_decode": (ci, [vp, vp, ci, ci, ci, vp, vp, vp]),
     "frcnn_detect_post_workspace_bytes": (sz, [ci, ci, ci]),
     "frcnn_detect_post": (ci, [vp, vp, vp, ci, ci, ci, cf, cf, cu, ci, ci, vp, vp, ci, vp, vp, vp, vp, sz, vp]),
+    "frcnn_detect_features": (ci, [vp, vp, vp, ci, ci, ci, ci, ci, vp, vp, vp]),
+    "frcnn_boxes_to_rois": (ci, [vp, vp, vp, ci, ci, vp, vp, vp]),
 }
 
 _lib = None

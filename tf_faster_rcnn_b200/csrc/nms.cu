@@ -394,6 +394,64 @@ cap_emit_kernel(const float4* __restrict__ pred, int r, int C, int max_per_image
   }
 }
 
+// ---- per-detection head features ---------------------------------------------------------------------------
+// Runs after cap_emit_kernel and rebuilds its slot order from the truncated keep lists (classes ascending, slot =
+// prefix(keep_cnt)[c] + j), so slot k of the features is record row k.  One CTA per (block of FEAT_SLOTS slots, image):
+// each thread scans 4 consecutive class counts (C <= 1024), then the CTA copies its slots' fc7 rows, float4 wide.
+constexpr int FEAT_THREADS = 256;
+constexpr int FEAT_SLOTS = 8;
+
+__global__ void __launch_bounds__(FEAT_THREADS)
+detect_features_kernel(const int* __restrict__ keep, const int* __restrict__ keep_cnt, const float4* __restrict__ fc7, int r, int C,
+                       int f4, int max_det, float4* __restrict__ feat_out, int* __restrict__ roi_out) {
+  __shared__ int s_off[1025];
+  __shared__ int s_warp[FEAT_THREADS / 32];
+  __shared__ int s_roi[FEAT_SLOTS];
+  const int img = blockIdx.y, slot0 = blockIdx.x * FEAT_SLOTS;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  keep += (size_t)img * C * r; keep_cnt += (size_t)img * C;
+  int cnt[4], v = 0;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const int c = 4 * tid + q;
+    cnt[q] = (c >= 1 && c < C) ? __ldg(keep_cnt + c) : 0;     // class 0 (background) never emits
+    v += cnt[q];
+  }
+  int incl = v;
+  for (int o = 1; o < 32; o <<= 1) { const int n = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += n; }
+  if (lane == 31) s_warp[warp] = incl;
+  __syncthreads();
+  int run = incl - v;
+  for (int w = 0; w < warp; ++w) run += s_warp[w];
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const int c = 4 * tid + q;
+    if (c < C) s_off[c] = run;
+    run += cnt[q];
+  }
+  if (tid == FEAT_THREADS - 1) s_off[C] = run;                  // detections of the image (the record's ndet)
+  __syncthreads();
+  if (tid < FEAT_SLOTS) {
+    const int slot = slot0 + tid;
+    int roi = -1;
+    if (slot < max_det && slot < s_off[C]) {
+      int lo = 1, hi = C;                                       // last class c with s_off[c] <= slot
+      while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (s_off[mid] <= slot) lo = mid; else hi = mid; }
+      roi = __ldg(keep + (size_t)lo * r + (slot - s_off[lo]));
+    }
+    s_roi[tid] = roi;
+    if (slot < max_det) roi_out[(size_t)img * max_det + slot] = roi;
+  }
+  __syncthreads();
+  const float4* src = fc7 + (size_t)img * r * f4;
+  for (int i = tid; i < FEAT_SLOTS * f4; i += FEAT_THREADS) {
+    const int s = i / f4, k = i - s * f4, slot = slot0 + s;
+    if (slot >= max_det) break;
+    const int roi = s_roi[s];
+    feat_out[((size_t)img * max_det + slot) * f4 + k] = roi >= 0 ? __ldg(src + (size_t)roi * f4 + k) : make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+}
+
 }  // namespace frcnn
 
 using namespace frcnn;
@@ -510,6 +568,21 @@ extern "C" int frcnn_detect_post(const float* cls_prob, const float* pred_boxes,
   cap_emit_kernel<<<(unsigned)batch, NMS_THREADS, 0, st>>>(reinterpret_cast<const float4*>(pred_boxes), r, num_classes, max_per_image, max_det,
                                                           keep, keep_cnt, keep_score, det, ndet,
                                                           record_stride ? record_stride : max_det * 6, record_stride ? record_stride : 1);
+  FRCNN_LAUNCH_CHECK();
+  return OK;
+}
+
+extern "C" int frcnn_detect_features(const int* keep, const int* keep_cnt, const float* fc7, int r, int batch, int num_classes,
+                                     int feat_dim, int max_det, float* feat_out, int* roi_out, void* stream) {
+  FRCNN_REQUIRE(keep && keep_cnt && fc7 && feat_out && roi_out, "detect_features: null pointer");
+  FRCNN_REQUIRE(r > 0 && batch > 0 && num_classes >= 2 && num_classes <= 1024 && max_det > 0,
+                "detect_features: r>0, batch>0, 2<=C<=1024, max_det>0 required");
+  FRCNN_REQUIRE(feat_dim > 0 && feat_dim % 4 == 0 && ((uintptr_t)fc7 & 15) == 0 && ((uintptr_t)feat_out & 15) == 0,
+                "detect_features: feat_dim %d must be a positive multiple of 4 and fc7 / feat_out 16-byte aligned", feat_dim);
+  const dim3 grid((unsigned)cdiv(max_det, FEAT_SLOTS), (unsigned)batch);
+  detect_features_kernel<<<grid, FEAT_THREADS, 0, (cudaStream_t)stream>>>(keep, keep_cnt, reinterpret_cast<const float4*>(fc7), r,
+                                                                         num_classes, feat_dim / 4, max_det,
+                                                                         reinterpret_cast<float4*>(feat_out), roi_out);
   FRCNN_LAUNCH_CHECK();
   return OK;
 }

@@ -382,6 +382,26 @@ __global__ void bbox_decode_kernel(const float* __restrict__ rois, const float* 
   reinterpret_cast<float4*>(pred)[i] = o;
 }
 
+// caller boxes (original-image pixels) -> RoI rows (image, x1*s, y1*s, x2*s, y2*s) in blob pixels, thread per (image, row).
+// Scale and count are read from device memory, so one captured graph serves every call of the same capacity.  No clipping:
+// crop_and_resize extrapolates samples outside the feature map to 0.
+__global__ void boxes_to_rois_kernel(const float4* __restrict__ boxes, const int* __restrict__ counts, const float* __restrict__ im_meta,
+                                     int batch, int cap, float* __restrict__ rois, int* __restrict__ num_rois) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= batch * cap) return;
+  const int b = i / cap, j = i - b * cap;
+  const int n = min(max(__ldg(counts + b), 0), cap);
+  if (j == 0) num_rois[b] = n;
+  float* row = rois + (size_t)i * 5;
+  if (j < n) {
+    const float s = __ldg(im_meta + b * 3);
+    const float4 bx = __ldg(boxes + i);
+    row[0] = (float)b; row[1] = __fmul_rn(bx.x, s); row[2] = __fmul_rn(bx.y, s); row[3] = __fmul_rn(bx.z, s); row[4] = __fmul_rn(bx.w, s);
+  } else {
+    row[0] = row[1] = row[2] = row[3] = row[4] = 0.f;
+  }
+}
+
 // ---- image -> blob on the device (SURVEY 8(f) rank 2): mean subtraction + cv2.resize(INTER_LINEAR) restated ----------
 // lib/model/test.py:35-36 (float32(pixel) - PIXEL_MEANS, evaluated in double and rounded once, as numpy's in-place
 // float32 -= float64 does) followed by OpenCV's float bilinear resize: source coordinate (dx + 0.5) / fx - 0.5 in double,
@@ -536,6 +556,16 @@ extern "C" int frcnn_bbox_decode(const float* rois, const float* bbox_pred, int 
   FRCNN_REQUIRE(rois && bbox_pred && pred_boxes && im_meta_dev && batch > 0, "bbox_decode: bad argument");
   bbox_decode_kernel<<<blocks_for((long)r * num_classes, 256), 256, 0, (cudaStream_t)stream>>>(rois, bbox_pred, r, num_classes, batch,
                                                                                              im_meta_dev, pred_boxes);
+  FRCNN_LAUNCH_CHECK();
+  return OK;
+}
+
+extern "C" int frcnn_boxes_to_rois(const float* boxes, const int* counts, const float* im_meta_dev, int batch, int cap, float* rois,
+                                   int* num_rois, void* stream) {
+  FRCNN_REQUIRE(boxes && counts && im_meta_dev && rois && num_rois, "boxes_to_rois: null pointer");
+  FRCNN_REQUIRE(batch > 0 && cap > 0 && ((uintptr_t)boxes & 15) == 0, "boxes_to_rois: batch>0, cap>0 and 16-byte aligned boxes required");
+  boxes_to_rois_kernel<<<blocks_for((long)batch * cap, 256), 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const float4*>(boxes), counts,
+                                                                                           im_meta_dev, batch, cap, rois, num_rois);
   FRCNN_LAUNCH_CHECK();
   return OK;
 }

@@ -206,9 +206,12 @@ class ShapePlan:
     backbone sees M = batch * H * W output pixels per layer (the 38x50 ResNet maps fill the 132 SMs without split-K), the
     per-RoI head sees batch * R RoIs, and the single-CTA proposal / NMS kernels run one CTA per image side by side.
     One image (or batch) = ONE graph replay: the im_detect / test_net tail is part of the graph, its per-image scalars
-    (scale, original size) are read from `im_meta` on the device."""
+    (scale, original size) are read from `im_meta` on the device.
 
-    def __init__(self, net, h, w, batch=1, use_graph=True):
+    rois_source="boxes" (the Fast R-CNN mode, TEST.HAS_RPN = False): the RoIs are `cap` caller boxes per image staged by
+    set_boxes() instead of the RPN's proposals; the RPN is not built and the head / im_detect tail are the same steps."""
+
+    def __init__(self, net, h, w, batch=1, use_graph=True, rois_source="rpn", cap=None):
         self.net, self.h, self.w, self.batch = net, h, w, batch
         cfgd = net.options
         wts = net.weights
@@ -217,14 +220,98 @@ class ShapePlan:
         B = batch
         self.image = t.new(B, h, w, 3)
         self.im_info = np.zeros(3, F)
-        A = net.num_anchors
         C = net.num_classes
         sc = net.scope
+        # per-image (scale, orig_h, orig_w), read by bbox_decode (and boxes_to_rois).  Pinned staging for the meta rows: a ring,
+        # because the H2D copies are asynchronous and the host may already be preparing the launch after next (submit_batch
+        # keeps two batches in flight)
+        self.im_meta = t.new(B, 3)
+        self.im_meta_ring = [torch.empty((B, 3), dtype=torch.float32).pin_memory() for _ in range(4)]
+        self.im_meta_turn = 0
+        self.im_meta_ring[0][:] = torch.tensor([1.0, float(h), float(w)])
+        self.im_meta.copy_(self.im_meta_ring[0])
         # ---- backbone -----------------------------------------------------------------------------------
         feat = net._image_to_head(t, self.image)
         self.feat = feat
         _, fh, fw, cb = feat.shape
         assert fh == -(-h // 16) and fw == -(-w // 16), "feature map %dx%d does not match ceil(H/16) x ceil(W/16)" % (fh, fw)
+        if rois_source == "boxes":
+            self._caller_rois(t, cap)
+        else:
+            self._rpn_rois(t, feat)
+        R = self.R
+        # ---- RoI pooling (network.py:141-157 / resnet_v1.py:55-76) ---------------------------------------
+        P = cfgd["pooling_size"]
+        pre_pool = net.crop_pre_pool()
+        self.pool5 = t.new(B * R, P, P, cb)
+        t.add("crop_pool", lambda: ops.crop_pool(feat, self.rois, P, pre_pool, self.pool5))
+        # ---- per-RoI head + fused cls_score|bbox_pred FC (network.py:361-378) ------------------------------
+        fc7 = net._head_to_tail(t, self.pool5)
+        self.fc7 = fc7
+
+        ld_head = (5 * C + 3) // 4 * 4            # zero-padded to a multiple of 4 columns: vector stores + split-K apply
+
+        def fused_cls():
+            wc, wb = wts[sc + "/cls_score/weights"], wts[sc + "/bbox_pred/weights"]
+            wf = np.zeros((1, 1, wc.shape[0], ld_head), F); bf = np.zeros(ld_head, F)
+            wf[0, 0, :, :C] = wc; wf[0, 0, :, C:5 * C] = wb
+            bf[:C] = wts[sc + "/cls_score/biases"]; bf[C:5 * C] = wts[sc + "/bbox_pred/biases"]
+            return wf, None, bf
+        self.head_out = t.fc(fc7, sc + "/cls_bbox", N.ACT_NONE, packed=wts.packed_custom(sc + "/cls_bbox", fused_cls))
+        self.cls_score = t.new(B * R, C); self.cls_prob = t.new(B * R, C); self.bbox_pred = t.new(B * R, 4 * C)
+        stds, means = cfgd["bbox_stds"], cfgd["bbox_means"]
+        t.add("cls_finish", lambda: ops.cls_finish(self.head_out, C, stds, means, self.cls_score, self.cls_prob, self.bbox_pred))
+        self.n_test_image_steps = len(t.steps)
+        # ---- im_detect tail on the device (test.py:95-107): per-image (scale, orig_h, orig_w) live in im_meta --------------
+        self.pred_boxes = t.new(B * R, 4 * C)
+        t.add("bbox_decode", lambda: ops.bbox_decode(self.rois, self.bbox_pred, C, self.im_meta, self.pred_boxes))
+        self.n_im_detect_steps = len(t.steps)
+        # ---- test_net tail (test.py:162-180): built on first use for the options in force (_ensure_post) ---------------------
+        self.keep = t.new(B, C, R, dtype=torch.int32); self.keep_cnt = t.new(B, C, dtype=torch.int32)
+        self.keep_score = t.new(B, C, R)
+        self.post_ws = ops.detect_post_workspace(R, C, B); t.bufs.append(self.post_ws)
+        self.post_key = None
+        self.recs = [None, None]       # two record buffers; `double_buffer` makes consecutive detect launches alternate
+        self.rec = self.det = self.ndet = None   # ... views of the buffer the LAST detect launch wrote
+        self.post_steps = [None, None]
+        self.feat_out = self.roi_out = self.features_step = None   # feature mode (_ensure_post(features=True))
+        self.double_buffer = False
+        self.slot = 0
+        self.max_det = 0
+        self.graphs = {}
+        self.use_graph = use_graph
+
+    def _caller_rois(self, t, cap):
+        """RoIs from caller boxes: [batch, cap, 4] boxes + int32 counts staged through a pinned ring (set_boxes)."""
+        B = self.batch
+        self.R = cap
+        self.rpn_out = self.rpn_dcol = self.roi_scores = self.roi_keep = None
+        self.boxes = t.new(B, cap, 4); self.box_counts = t.new(B, dtype=torch.int32)
+        self.box_ring = [(torch.zeros((B, cap, 4), dtype=torch.float32).pin_memory(), torch.zeros(B, dtype=torch.int32).pin_memory())
+                         for _ in range(4)]
+        self.box_turn = 0
+        self.box_counts.zero_()
+        self.rois = t.new(B * cap, 5); self.num_rois = t.new(B, dtype=torch.int32)
+        t.add("boxes_to_rois", lambda: ops.boxes_to_rois(self.boxes, self.box_counts, self.im_meta, self.rois, self.num_rois))
+
+    def set_boxes(self, boxes):
+        """boxes: per image an fp32 [n_i, 4] array (original-image pixels, n_i <= cap); staged in pinned memory and copied on
+        the launching stream, like set_meta."""
+        self.box_turn = (self.box_turn + 1) & 3
+        hb, hc = self.box_ring[self.box_turn]
+        for b, a in enumerate(boxes):
+            n = a.shape[0]
+            hc[b] = n
+            if n:
+                hb[b, :n] = torch.from_numpy(a)
+        self.boxes.copy_(hb, non_blocking=True)
+        self.box_counts.copy_(hc, non_blocking=True)
+
+    def _rpn_rois(self, t, feat):
+        """RoIs from the RPN: 3x3 conv, fused cls|bbox 1x1, decode, sort, proposal NMS."""
+        net, B, h, w = self.net, self.batch, self.h, self.w
+        cfgd, wts, sc, A = net.options, net.weights, net.scope, net.num_anchors
+        _, fh, fw, _ = feat.shape
         # ---- RPN (network.py:323-359): 3x3 conv + ONE fused 1x1 for cls(2A) | pad | bbox(4A) ---------------
         rpn = t.conv(feat, sc + "/rpn_conv/3x3", 1, "SAME", N.ACT_RELU)
         dcol = (2 * A + 3) // 4 * 4
@@ -260,52 +347,6 @@ class ShapePlan:
         self.roi_keep = t.new(B * R, dtype=torch.int32); self.num_rois = t.new(B, dtype=torch.int32)
         t.add("proposals", lambda: ops.proposals(self.rpn_props, self.rpn_scores, self.order, pre, R, thr, flags, self.rois,
                                                  self.roi_scores, self.roi_keep, self.num_rois, batch=B))
-        # ---- RoI pooling (network.py:141-157 / resnet_v1.py:55-76) ---------------------------------------
-        P = cfgd["pooling_size"]
-        pre_pool = net.crop_pre_pool()
-        self.pool5 = t.new(B * R, P, P, cb)
-        t.add("crop_pool", lambda: ops.crop_pool(feat, self.rois, P, pre_pool, self.pool5))
-        # ---- per-RoI head + fused cls_score|bbox_pred FC (network.py:361-378) ------------------------------
-        fc7 = net._head_to_tail(t, self.pool5)
-        self.fc7 = fc7
-
-        ld_head = (5 * C + 3) // 4 * 4            # zero-padded to a multiple of 4 columns: vector stores + split-K apply
-
-        def fused_cls():
-            wc, wb = wts[sc + "/cls_score/weights"], wts[sc + "/bbox_pred/weights"]
-            wf = np.zeros((1, 1, wc.shape[0], ld_head), F); bf = np.zeros(ld_head, F)
-            wf[0, 0, :, :C] = wc; wf[0, 0, :, C:5 * C] = wb
-            bf[:C] = wts[sc + "/cls_score/biases"]; bf[C:5 * C] = wts[sc + "/bbox_pred/biases"]
-            return wf, None, bf
-        self.head_out = t.fc(fc7, sc + "/cls_bbox", N.ACT_NONE, packed=wts.packed_custom(sc + "/cls_bbox", fused_cls))
-        self.cls_score = t.new(B * R, C); self.cls_prob = t.new(B * R, C); self.bbox_pred = t.new(B * R, 4 * C)
-        stds, means = cfgd["bbox_stds"], cfgd["bbox_means"]
-        t.add("cls_finish", lambda: ops.cls_finish(self.head_out, C, stds, means, self.cls_score, self.cls_prob, self.bbox_pred))
-        self.n_test_image_steps = len(t.steps)
-        # ---- im_detect tail on the device (test.py:95-107): per-image (scale, orig_h, orig_w) live in im_meta --------------
-        self.pred_boxes = t.new(B * R, 4 * C)
-        self.im_meta = t.new(B, 3)
-        # pinned staging for the meta rows: a ring, because the H2D copies are asynchronous and the host may already be
-        # preparing the launch after next (submit_batch keeps two batches in flight)
-        self.im_meta_ring = [torch.empty((B, 3), dtype=torch.float32).pin_memory() for _ in range(4)]
-        self.im_meta_turn = 0
-        self.im_meta_ring[0][:] = torch.tensor([1.0, float(h), float(w)])
-        self.im_meta.copy_(self.im_meta_ring[0])
-        t.add("bbox_decode", lambda: ops.bbox_decode(self.rois, self.bbox_pred, C, self.im_meta, self.pred_boxes))
-        self.n_im_detect_steps = len(t.steps)
-        # ---- test_net tail (test.py:162-180): built on first use for the options in force (_ensure_post) ---------------------
-        self.keep = t.new(B, C, R, dtype=torch.int32); self.keep_cnt = t.new(B, C, dtype=torch.int32)
-        self.keep_score = t.new(B, C, R)
-        self.post_ws = ops.detect_post_workspace(R, C, B); t.bufs.append(self.post_ws)
-        self.post_key = None
-        self.recs = [None, None]       # two record buffers; `double_buffer` makes consecutive detect launches alternate
-        self.rec = self.det = self.ndet = None   # ... views of the buffer the LAST detect launch wrote
-        self.post_steps = [None, None]
-        self.double_buffer = False
-        self.slot = 0
-        self.max_det = 0
-        self.graphs = {}
-        self.use_graph = use_graph
 
     def nbytes(self):
         return sum(b.numel() * b.element_size() for b in self.tape.bufs)
@@ -319,14 +360,25 @@ class ShapePlan:
         self.post_steps = [None, None]
         self.recs = [None, None]
         self.rec = self.det = self.ndet = None
+        self.feat_out = self.roi_out = self.features_step = None
 
-    def _ensure_post(self):
-        """(Re)build the detection-record buffers and the post step for the current score / NMS thresholds and cap."""
-        net = self.net
-        o = net.options
+    def _ensure_post(self, features=False):
+        """(Re)build the detection-record buffers and the post step for the current score / NMS thresholds and cap; with
+        `features`, also the per-detection feature buffers and their gather step."""
+        o = self.net.options
         key = (float(o["score_thresh"]), float(o["nms_thresh"]), bool(o["use_gpu_nms"]), int(o["max_per_image"]))
-        if key == self.post_key:
-            return
+        if key != self.post_key:
+            self._build_post(key)
+        if features and self.features_step is None:
+            check_feature_mode(key[3])
+            C, B, fdim = self.net.num_classes, self.batch, int(self.fc7.shape[1])
+            # feat_out [B, max_det, F]: row k of image b = fc7 row of record row k; roi_out [B, max_det] int32 (-1 past the count)
+            self.feat_out = ops.zeros((B, self.max_det, fdim))
+            self.roi_out = ops.zeros((B, self.max_det), dtype=torch.int32)
+            self.features_step = lambda: ops.detect_features(self.keep, self.keep_cnt, self.fc7, C, self.feat_out, self.roi_out)
+
+    def _build_post(self, key):
+        net = self.net
         C, R, B = net.num_classes, self.R, self.batch
         mpi = key[3]
         # records: max_per_image survivors + head-room for ties at the threshold score; no cap -> every (roi, class) pair.
@@ -347,6 +399,8 @@ class ShapePlan:
         self.post_key = key
         self._select(0)
         self.graphs.pop(("detect", 0), None); self.graphs.pop(("detect", 1), None)
+        self.feat_out = self.roi_out = self.features_step = None
+        self.graphs.pop(("features", 0), None)
 
     def _select(self, slot):
         self.slot = slot
@@ -355,13 +409,16 @@ class ShapePlan:
         self.ndet = self.rec.view(torch.int32)[:, 0]
 
     def steps_for(self, mode):
-        """mode: 'test_image' (network outputs), 'im_detect' (+ decoded boxes), 'detect' (+ per-class NMS, cap, records)."""
+        """mode: 'test_image' (network outputs), 'im_detect' (+ decoded boxes), 'detect' (+ per-class NMS, cap, records),
+        'features' (+ the head feature and RoI index of every record row)."""
         if mode == "test_image":
             return [fn for _, fn in self.tape.steps[:self.n_test_image_steps]]
         fns = [fn for _, fn in self.tape.steps[:self.n_im_detect_steps]]
-        if mode == "detect":
-            self._ensure_post()
+        if mode in ("detect", "features"):
+            self._ensure_post(features=mode == "features")
             fns.append(self.post_steps[self.slot])
+        if mode == "features":
+            fns.append(self.features_step)
         return fns
 
     def set_meta(self, rows):
@@ -372,19 +429,20 @@ class ShapePlan:
             host[b, 0] = float(F(s)); host[b, 1] = float(oh); host[b, 2] = float(ow)
         self.im_meta.copy_(host, non_blocking=True)
 
-    def launch(self, im_scale=1.0, orig_h=None, orig_w=None, post=False, detect=False, meta=None):
+    def launch(self, im_scale=1.0, orig_h=None, orig_w=None, post=False, detect=False, meta=None, features=False):
         """Enqueue one batch (inputs already in self.image) on the current stream.  meta: per-image (scale, orig_h, orig_w)
-        rows; the scalar arguments describe every image of the batch when meta is None."""
-        mode = "detect" if detect else ("im_detect" if post else "test_image")
+        rows; the scalar arguments describe every image of the batch when meta is None.  features: detect + the feature
+        gather into feat_out / roi_out (always record buffer 0: feature mode does not double-buffer)."""
+        mode = "features" if features else "detect" if detect else ("im_detect" if post else "test_image")
         if mode != "test_image":
             if meta is None:
                 meta = [(im_scale, orig_h if orig_h is not None else self.h, orig_w if orig_w is not None else self.w)] * self.batch
             self.set_meta(meta)
         gkey = mode
-        if mode == "detect":
-            self._ensure_post()
-            self._select(self.slot ^ 1 if self.double_buffer else 0)
-            gkey = ("detect", self.slot)
+        if mode in ("detect", "features"):
+            self._ensure_post(features=features)
+            self._select(self.slot ^ 1 if self.double_buffer and not features else 0)
+            gkey = (mode, self.slot)
         if self.use_graph:
             g = self.graphs.get(gkey)
             if g is None:
@@ -415,6 +473,38 @@ def split_host_records(host, max_det):
                                "(score ties beyond the max_per_image head-room)" % (b, n, max_det))
         out.append(host[b, REC_HEADER:REC_HEADER + n * 6].view(n, 6).numpy().copy())
     return out
+
+
+BOX_CAPACITIES = (64, 128, 256, 512, 1024)   # caller-box plans are built per (shape, batch, capacity): few distinct graphs
+
+
+def box_capacity(n):
+    """Smallest capacity in BOX_CAPACITIES that holds n caller boxes per image."""
+    for cap in BOX_CAPACITIES:
+        if n <= cap:
+            return cap
+    raise ValueError("%d boxes for one image: at most %d per call, split them over several calls" % (n, BOX_CAPACITIES[-1]))
+
+
+def check_boxes(boxes, batch):
+    """Caller boxes: a list of `batch` fp32 [n_i, 4] arrays (x1, y1, x2, y2 in original-image pixels) -> contiguous copies."""
+    if len(boxes) != batch:
+        raise ValueError("%d box arrays for %d images" % (len(boxes), batch))
+    out = []
+    for i, b in enumerate(boxes):
+        a = b.numpy() if isinstance(b, torch.Tensor) else np.asarray(b)
+        if a.ndim != 2 or a.shape[1] != 4:
+            raise ValueError("boxes[%d] has shape %s, expected [n, 4]" % (i, tuple(a.shape)))
+        if a.dtype != np.float32:
+            raise TypeError("boxes[%d] has dtype %s, expected float32" % (i, a.dtype))
+        out.append(np.ascontiguousarray(a))
+    return out
+
+
+def check_feature_mode(max_per_image):
+    if max_per_image <= 0:
+        raise ValueError("per-detection features need max_per_image > 0: without the cap the record buffer holds every "
+                         "(RoI, class) pair, R*(C-1) feature rows per image (hundreds of MB)")
 
 
 def nms_threshold(thresh, use_gpu_nms):

@@ -57,13 +57,16 @@ def blob_geometry(im_shape):
     return int(np.rint(im_shape[0] * f)), int(np.rint(im_shape[1] * f)), f
 
 
-def _run_device_preprocess(net, im, post, detect):
-    """uint8 image -> H2D (0.5 MB instead of the 5.8 MB fp32 blob) -> preprocess kernel -> graph."""
-    from tf_faster_rcnn_b200 import ops
+def _run_device_preprocess(net, im, post, detect, boxes=None):
+    """uint8 image -> H2D (0.5 MB instead of the 5.8 MB fp32 blob) -> preprocess kernel -> graph.  boxes: caller RoIs
+    (fp32 [n,4], original-image pixels) instead of the RPN's."""
+    from tf_faster_rcnn_b200 import ops, engine
     H, W, f = blob_geometry(im.shape)
-    plan = net.plan_for(H, W)
+    plan = net.plan_for(H, W) if boxes is None else net.plan_for(H, W, cap=engine.box_capacity(boxes.shape[0]))
     img = torch.from_numpy(np.ascontiguousarray(im)).cuda(non_blocking=True)
     ops.preprocess(img, np.asarray(cfg.PIXEL_MEANS, dtype=np.float64).ravel(), f, f, plan.image)
+    if boxes is not None:
+        plan.set_boxes([boxes])
     plan.launch(f, im.shape[0], im.shape[1], post=post, detect=detect)
     return plan, f
 
@@ -73,17 +76,25 @@ def _get_blobs(im):
     return {'data': data}, factors
 
 
-def im_detect(sess, net, im):
-    """-> scores [R, C] fp32, pred_boxes [R, 4C] fp32 in ORIGINAL-image pixels."""
+def im_detect(sess, net, im, boxes=None):
+    """-> scores [R, C] fp32, pred_boxes [R, 4C] fp32 in ORIGINAL-image pixels.  boxes: [n, 4] boxes (x1,y1,x2,y2,
+    original-image pixels) scored instead of the RPN's proposals (Fast R-CNN, TEST.HAS_RPN = False): then R = n, in the
+    given order."""
+    if boxes is not None:
+        from tf_faster_rcnn_b200 import engine
+        boxes = engine.check_boxes([np.asarray(boxes, dtype=np.float32)], 1)[0]
     if DEVICE_PREPROCESS:
-        plan, f = _run_device_preprocess(net, im, post=True, detect=False)
+        plan, f = _run_device_preprocess(net, im, post=True, detect=False, boxes=boxes)
         im_scales = np.array([f])
     else:
         blobs, im_scales = _get_blobs(im)
         assert len(im_scales) == 1, "Only single-image batch implemented"
         blob = blobs['data']
         blobs['im_info'] = np.array([blob.shape[1], blob.shape[2], im_scales[0]], dtype=np.float32)
-        plan = net._run(blob, blobs['im_info'], post=True, detect=False, orig_hw=im.shape[:2])
+        if boxes is None:
+            plan = net._run(blob, blobs['im_info'], post=True, detect=False, orig_hw=im.shape[:2])
+        else:
+            plan = net._run_boxes(blob, [im_scales[0]], [im.shape[:2]], [boxes])
     torch.cuda.current_stream().synchronize()
     r = int(plan.num_rois[0].item())
     scores = plan.cls_prob[:r].cpu().numpy()

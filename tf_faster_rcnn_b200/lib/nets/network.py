@@ -116,13 +116,14 @@ class Network(object):
 
     MAX_PLANS = int(os.environ.get("FRCNN_MAX_PLANS", "6"))
 
-    def plan_for(self, h, w, batch=1):
+    def plan_for(self, h, w, batch=1, cap=None):
         """ShapePlan of blob shape (h, w) x batch.  A plan owns every layer's activation buffer, the TMA descriptors and the CUDA
         graphs of that shape (0.6-1.3 GB per image at 600x800..1000), so the cache is a small LRU: a dataset with hundreds of
-        distinct shapes recycles plans instead of growing without bound (evicted buffers return to the caching allocator)."""
+        distinct shapes recycles plans instead of growing without bound (evicted buffers return to the caching allocator).
+        cap: a caller-box plan (RoIs = up to `cap` given boxes per image, no RPN), cached beside the RPN plans."""
         if self.weights is None:
             raise RuntimeError("no weights loaded: call load_weights() / Saver.restore() before test_image")
-        key = (int(h), int(w), int(batch))
+        key = (int(h), int(w), int(batch)) if cap is None else (int(h), int(w), int(batch), "boxes", int(cap))
         plan = self._plans.pop(key, None)
         if plan is None:
             dev = torch.cuda.current_device() if torch.cuda.is_available() else 0
@@ -132,7 +133,8 @@ class Network(object):
                 old = self._plans.pop(old_key)
                 torch.cuda.current_stream().synchronize()   # nothing of the evicted plan is still in flight
                 old.release()
-            plan = engine.ShapePlan(self, key[0], key[1], key[2], use_graph=self.use_cuda_graph)
+            plan = engine.ShapePlan(self, key[0], key[1], key[2], use_graph=self.use_cuda_graph,
+                                    rois_source="rpn" if cap is None else "boxes", cap=cap)
         self._plans[key] = plan                             # most recently used last
         return plan
 
@@ -165,6 +167,44 @@ class Network(object):
         self._copy_in(plan, images)
         plan.launch(post=True, detect=True, meta=[(float(im_scales[i]), int(orig_hws[i][0]), int(orig_hws[i][1])) for i in range(b)])
         return plan.records(), plan
+
+    # ---- region features: per-detection head features, and scoring of caller-supplied boxes ---------------------------------
+    def detect_features(self, images, im_scales, orig_hws):
+        """detect_batch plus, for every detection, the head's per-RoI feature vector (fc7: 2048-d ResNet, 4096-d VGG16, 1024-d
+        MobileNet) and the index of the RoI it came from, gathered on the device in the same graph replay.
+        -> (list over images of (det [n,6], feats [n,F] fp32, roi_index [n] int32), plan); det equals detect_batch's records.
+        Needs options['max_per_image'] > 0."""
+        b = int(images.shape[0])
+        assert images.shape[3] == 3 and len(im_scales) == b and len(orig_hws) == b
+        engine.check_feature_mode(int(self.options["max_per_image"]))
+        plan = self.plan_for(images.shape[1], images.shape[2], b)
+        self._copy_in(plan, images)
+        plan.launch(post=True, features=True, meta=[(float(im_scales[i]), int(orig_hws[i][0]), int(orig_hws[i][1])) for i in range(b)])
+        dets = plan.records()
+        feats, rois = plan.feat_out.cpu(), plan.roi_out.cpu()
+        return [(d, feats[i, :d.shape[0]].numpy().copy(), rois[i, :d.shape[0]].numpy().copy()) for i, d in enumerate(dets)], plan
+
+    def _run_boxes(self, images, im_scales, orig_hws, boxes):
+        """Enqueue `images` [B,H,W,3] with caller boxes as the RoIs on a caller-box plan (no sync) -> plan."""
+        b = int(images.shape[0])
+        assert images.shape[3] == 3 and len(im_scales) == b and len(orig_hws) == b
+        boxes = engine.check_boxes(boxes, b)
+        plan = self.plan_for(images.shape[1], images.shape[2], b, cap=engine.box_capacity(max(a.shape[0] for a in boxes)))
+        self._copy_in(plan, images)
+        plan.set_boxes(boxes)
+        plan.launch(post=True, meta=[(float(im_scales[i]), int(orig_hws[i][0]), int(orig_hws[i][1])) for i in range(b)])
+        return plan
+
+    def score_boxes(self, images, im_scales, orig_hws, boxes):
+        """The Fast R-CNN mode: classify and regress caller boxes instead of RPN proposals.  boxes: per image an fp32 [n_i, 4]
+        array (x1, y1, x2, y2 in original-image pixels, n_i <= 1024).  -> (list over images of (scores [n_i, C],
+        pred_boxes [n_i, 4C], feats [n_i, F]), plan): im_detect's outputs for those boxes, plus the head features."""
+        plan = self._run_boxes(images, im_scales, orig_hws, boxes)
+        out = []
+        for i, a in enumerate(boxes):
+            rows = slice(i * plan.R, i * plan.R + a.shape[0])
+            out.append((plan.cls_prob[rows].cpu().numpy(), plan.pred_boxes[rows].cpu().numpy(), plan.fc7[rows].cpu().numpy()))
+        return out, plan
 
     # ---- pipelined throughput API: overlap the next batch's host->device copy with the current batch's compute ---------------
     def submit_batch(self, images, im_scales, orig_hws):

@@ -229,6 +229,22 @@ def detect_post(cls_prob, pred_boxes, num_rois, num_classes, score_thresh, nms_t
                                       _stream()), "detect_post")
 
 
+def detect_features(keep, keep_cnt, fc7, num_classes, feat_out, roi_out):
+    """After detect_post: keep [batch, C, r], keep_cnt [batch, C] (the capped lists), fc7 [batch*r, F] ->
+    feat_out [batch, max_det, F] = fc7 row of record slot k, roi_out int32 [batch, max_det] (-1 past the count)."""
+    batch, max_det, fdim = feat_out.shape
+    r = keep.shape[-1]
+    N.check(N.lib().frcnn_detect_features(_p(keep), _p(keep_cnt), _p(_f32(fc7)), r, batch, num_classes, fdim, max_det, _p(_f32(feat_out)),
+                                          _p(roi_out), _stream()), "detect_features")
+
+
+def boxes_to_rois(boxes, counts, im_meta, rois, num_rois):
+    """boxes [batch, cap, 4] original-image pixels, counts int32 [batch], im_meta [batch, 3] -> rois [batch*cap, 5], num_rois."""
+    batch, cap, _ = boxes.shape
+    N.check(N.lib().frcnn_boxes_to_rois(_p(_f32(boxes)), _p(counts), _p(_f32(im_meta)), batch, cap, _p(_f32(rois)), _p(num_rois),
+                                        _stream()), "boxes_to_rois")
+
+
 def nms_sorted_dev(boxes, thresh, flags, max_out, keep, num):
     N.check(N.lib().frcnn_nms_sorted_dev(_p(_f32(boxes)), boxes.shape[0], float(thresh), flags, max_out, _p(keep), _p(num),
                                          _stream()), "nms_sorted_dev")

@@ -1,0 +1,104 @@
+#!/usr/bin/env python
+"""Region features ("bottom-up" features for captioning / VQA / grounding): one .npz per image of an imdb.
+
+    python tools/extract_features.py --imdb voc_2007_test --net res101 --model ckpt --out DIR [--batch B] [--boxes FILE.pkl]
+
+Without --boxes, each file holds the detector's final detections (per-class NMS + max_per_image cap, as test_net) and the
+head feature of the RoI each came from (2048-d ResNet, 4096-d VGG16, 1024-d MobileNet):
+    boxes [n,4] fp32 (x1,y1,x2,y2, image pixels), scores [n] fp32, classes [n] int32, features [n,F] fp32,
+    roi_index [n] int32 (RoI row within the image), image_h, image_w.
+With --boxes FILE.pkl (a dict image index -> [n,4] boxes in image pixels, or a list in imdb order), the given boxes are
+scored instead of RPN proposals (the Fast R-CNN mode):
+    boxes [n,4], scores [n,C] fp32 (class probabilities), features [n,F], image_h, image_w.
+Consecutive images whose blobs have the same shape are run together, up to --batch per device launch.  Without --model
+the network gets seeded synthetic weights."""
+import argparse
+import os
+import pickle
+import sys
+
+import _init_paths  # noqa: F401
+import cv2
+import numpy as np
+
+from datasets.factory import get_imdb
+from model.config import cfg_from_file, cfg_from_list
+from model.test import _get_blobs, _set_post_options
+from tools_common import build_net
+
+
+def parse_args(argv=None):
+    p = argparse.ArgumentParser(description="Per-region head features of a Faster R-CNN network on the H100 path")
+    p.add_argument("--imdb", dest="imdb_name", required=True)
+    p.add_argument("--net", default="res101", help="vgg16, res50, res101, res152, mobile")
+    p.add_argument("--model", default=None, help="TF checkpoint or .npz (default: seeded synthetic weights)")
+    p.add_argument("--batch", type=int, default=1, help="images per device launch (consecutive images of one blob shape)")
+    p.add_argument("--boxes", default=None, help="pickle of caller boxes per image: score these instead of detecting")
+    p.add_argument("--num_dets", dest="max_per_image", type=int, default=100)
+    p.add_argument("--out", required=True)
+    p.add_argument("--cfg", dest="cfg_file", default=None)
+    p.add_argument("--set", dest="set_cfgs", default=None, nargs=argparse.REMAINDER)
+    return p.parse_args(argv)
+
+
+def image_boxes(boxes, imdb, i):
+    if isinstance(boxes, dict):
+        key = imdb.image_index[i]
+        b = boxes[key] if key in boxes else boxes[i]
+    else:
+        b = boxes[i]
+    return np.asarray(b, dtype=np.float32).reshape(-1, 4)
+
+
+def extract(net, imdb, out_dir, batch=1, boxes=None, max_per_image=100):
+    """Writes <out_dir>/<image index>.npz for every image of `imdb`; returns the number of files written."""
+    _set_post_options(net, 0.0, max_per_image)
+    os.makedirs(out_dir, exist_ok=True)
+    group = []                                   # (image number, blob, scale, (h, w))
+
+    def flush():
+        blobs = np.concatenate([g[1] for g in group], axis=0)
+        scales, hws = [g[2] for g in group], [g[3] for g in group]
+        if boxes is None:
+            res, _ = net.detect_features(blobs, scales, hws)
+            for (i, _, _, hw), (det, feats, roi) in zip(group, res):
+                np.savez(os.path.join(out_dir, "%s.npz" % imdb.image_index[i]), boxes=det[:, :4], scores=det[:, 4],
+                         classes=det[:, 5].astype(np.int32), features=feats, roi_index=roi, image_h=hw[0], image_w=hw[1])
+        else:
+            given = [image_boxes(boxes, imdb, g[0]) for g in group]
+            res, _ = net.score_boxes(blobs, scales, hws, given)
+            for (i, _, _, hw), bx, (scores, _, feats) in zip(group, given, res):
+                np.savez(os.path.join(out_dir, "%s.npz" % imdb.image_index[i]), boxes=bx, scores=scores, features=feats,
+                         image_h=hw[0], image_w=hw[1])
+        del group[:]
+
+    for i in range(len(imdb.image_index)):
+        im = cv2.imread(imdb.image_path_at(i))
+        blobs, im_scales = _get_blobs(im)
+        blob = blobs["data"]
+        if group and (len(group) >= batch or group[0][1].shape != blob.shape):
+            flush()
+        group.append((i, blob, float(im_scales[0]), tuple(im.shape[:2])))
+    if group:
+        flush()
+    return len(imdb.image_index)
+
+
+def main(argv=None):
+    args = parse_args(argv)
+    if args.cfg_file is not None:
+        cfg_from_file(args.cfg_file)
+    if args.set_cfgs is not None:
+        cfg_from_list(args.set_cfgs)
+    imdb = get_imdb(args.imdb_name)
+    net = build_net(args.net, imdb.num_classes, args.model)
+    boxes = None
+    if args.boxes:
+        with open(args.boxes, "rb") as f:
+            boxes = pickle.load(f)
+    n = extract(net, imdb, args.out, max(1, args.batch), boxes, args.max_per_image)
+    print("wrote %d feature files to %s" % (n, args.out))
+
+
+if __name__ == "__main__":
+    sys.exit(main())
