@@ -88,10 +88,15 @@ int frcnn_nms_sorted_dev(const float* boxes_dev, int n, float thresh, unsigned f
  *                          * scale[co] + shift[co] (+ residual[n,ho,wo,co]) )
  * Requirements: cin % 32 == 0.  w_hi/w_lo from frcnn_pack_conv_weights.  scale may be NULL (=1). */
 typedef struct frcnn_conv_plan frcnn_conv_plan;
-#define FRCNN_CONV_F16X3 0   /* fp16 hi/lo split of both operands, 3 x wgmma f16, fp32 accumulate */
-#define FRCNN_CONV_TF32X3 1  /* tf32 hi/lo split, 3 x wgmma tf32 (same 22-bit products, twice the tensor time) */
-#define FRCNN_CONV_F16X1 2   /* THROUGHPUT mode, not fp32-grade: plain fp16 operands (the hi planes only), 1 MMA per product, fp32
-                              * accumulate; ~3e-4 of the output range per layer instead of ~4e-7.  Same packed weights as F16X3. */
+#define FRCNN_CONV_F16X3 0   /* fp16 hi/lo split of both operands, 3 x wgmma f16, fp32 accumulate.  Operands carried to 2^-22
+                              * relative for activations 2^-14 <= |x| < 65520 and weights down to 2^-27 below the layer's largest;
+                              * smaller activations lose precision (2^-20 at 2^-16, 2^-12 at 2^-24).  |x| >= 65520, +-Inf and NaN
+                              * make every output whose receptive field holds them non-finite. */
+#define FRCNN_CONV_TF32X3 1  /* tf32 hi/lo split, 3 x wgmma tf32 (same 22-bit products, twice the tensor time); 2^-22 relative from
+                              * 2^-115 up to the tf32 overflow, non-finite inputs give non-finite outputs */
+#define FRCNN_CONV_F16X1 2   /* THROUGHPUT mode, not fp32-grade: plain fp16 operands (the hi planes only, 2^-12 relative), 1 MMA per
+                              * product, fp32 accumulate; ~3e-4 of the output range per layer instead of ~4e-7.  Same packed
+                              * weights and the same activation range as F16X3. */
 
 typedef struct {
   const float* in_dev;       /* [n, h, w, cin] */

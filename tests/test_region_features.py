@@ -99,10 +99,15 @@ def test_oracle_score_boxes_reproduces_test_image_on_its_own_rois():
     assert np.array_equal(sb["pred_boxes"], want[1])
 
 
-@pytest.mark.parametrize("obj,kernel", [("nms", "detect_features_kernel"), ("simt_ops", "boxes_to_rois_kernel")])
+INSTANTIATIONS = {"conv_gemm_kernel": 6}      # 2 block_n x 3 arithmetic modes; every other kernel: 1
+
+
+@pytest.mark.parametrize("obj,kernel", [("nms", "detect_features_kernel"), ("simt_ops", "boxes_to_rois_kernel"),
+                                        ("conv_gemm", "conv_gemm_kernel")])
 def test_new_kernels_do_not_spill(obj, kernel):
-    """ptxas -v output written by the build (one log per object)."""
+    """ptxas -v output written by the build (one log per object), for every instantiation of the kernel."""
     log = open(os.path.join(ROOT, "tf_faster_rcnn_b200", "csrc", "_obj", obj + ".o.log")).read()
-    m = re.search(r"Function properties for \S*%s\S*\s*\n([^\n]*)" % kernel, log)
-    assert m, "no ptxas report for %s" % kernel
-    assert "0 bytes spill stores, 0 bytes spill loads" in m.group(1), m.group(1)
+    found = re.findall(r"Function properties for \S*%s\S*\s*\n([^\n]*)" % kernel, log)
+    assert len(found) == INSTANTIATIONS.get(kernel, 1), "ptxas reports for %s: %d" % (kernel, len(found))
+    for line in found:
+        assert "0 bytes spill stores, 0 bytes spill loads" in line, line

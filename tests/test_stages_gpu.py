@@ -28,48 +28,109 @@ def rand_boxes(rng, n, size=600.0, wh=(8, 200)):
 
 
 # ---------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("k,stride,cout,act,bn", [(3, 1, 64, 1, False), (7, 2, 64, 1, True), (3, 2, 32, 2, True)])
-def test_conv_first(cuda, k, stride, cout, act, bn):
+# SIMT convolutions: each output is one fixed-order chain of K fmaf from 0, then v*scale and + shift rounded once each, so
+# |got - y64| <= |scale| * gamma_K * S + u * (|v*scale| + |v*scale + shift|) per element (classical bound, gamma_K =
+# K u / (1 - K u), S = sum |x||w|; the activation is 1-Lipschitz).  The outputs sit in a NaN-prefilled view between
+# sentinel guard bands.
+U32 = 2.0 ** -24
+GUARD = 64
+SENTINEL = np.int32(0x7fa5a5a5)
+
+
+def gamma(k):
+    return k * U32 / (1 - k * U32)
+
+
+def guarded_out(shape):
+    numel = int(np.prod(shape))
+    buf = torch.full((numel + 2 * GUARD,), int(SENTINEL), dtype=torch.int32, device="cuda")
+    out = buf.view(torch.float32)[GUARD:GUARD + numel].view(shape)
+    out.fill_(float("nan"))
+    return buf, out
+
+
+def check_guarded(buf, numel):
+    b = buf.cpu().numpy()
+    assert (b[:GUARD] == SENTINEL).all() and (b[GUARD + numel:] == SENTINEL).all(), "store outside the output"
+
+
+def conv64_nhwc(x, w_oihw, stride, pt, pl, ho, wo, groups=1):
+    xt = torch.from_numpy(x.astype(np.float64)).permute(0, 3, 1, 2)
+    kh, kw = w_oihw.shape[2:]
+    pb = max((ho - 1) * stride + kh - x.shape[1] - pt, 0)
+    pr = max((wo - 1) * stride + kw - x.shape[2] - pl, 0)
+    xt = torch.nn.functional.pad(xt, (pl, pr, pt, pb))
+    y = torch.nn.functional.conv2d(xt, torch.from_numpy(w_oihw.astype(np.float64)), None, stride=stride, groups=groups)
+    return y.permute(0, 2, 3, 1).numpy()[:, :ho, :wo]
+
+
+def check_fma_chain(got, x, w_oihw, stride, pt, pl, ho, wo, K, scale, shift, act, groups=1):
+    v = conv64_nhwc(x, w_oihw, stride, pt, pl, ho, wo, groups)
+    S = conv64_nhwc(np.abs(x), np.abs(w_oihw), stride, pt, pl, ho, wo, groups)
+    sc = np.ones(v.shape[-1]) if scale is None else scale.astype(np.float64)
+    a = v * sc
+    b = a + shift.astype(np.float64)
+    y = np.maximum(b, 0) if act == 1 else np.minimum(np.maximum(b, 0), 6)
+    bound = (np.abs(sc) * gamma(K) * S + U32 * (np.abs(a) + np.abs(b))) * (1 + 4 * K * U32) + 1e-37
+    err = np.abs(got.astype(np.float64) - y)
+    assert np.isfinite(got).all(), "unwritten output"
+    assert (err <= bound).all(), "max err/bound %.3g" % (err / bound).max()
+    return float((err / bound).max())
+
+
+def with_batch(cases, ns=(1, 3)):
+    """Each case at batch 1 (id unchanged) and at the larger batches (id + '-n<batch>')."""
+    out = []
+    for c in cases:
+        c = c if isinstance(c, tuple) else (c,)
+        base = "-".join(str(v) for v in c)
+        out += [pytest.param(*c, n, id=base if n == 1 else "%s-n%d" % (base, n)) for n in ns]
+    return out
+
+
+# ResNet conv1 (7x7/2, BN), VGG conv1_1 (3x3/1, bias), MobileNet Conv2d_0 (3x3/2, BN, ReLU6); odd maps, partial tiles
+@pytest.mark.parametrize("k,stride,cout,act,bn,n", with_batch([(3, 1, 64, 1, False), (7, 2, 64, 1, True), (3, 2, 32, 2, True)]))
+def test_conv_first(cuda, k, stride, cout, act, bn, n):
     from tf_faster_rcnn_b200 import ops
-    rng = np.random.default_rng(k * 10 + stride)
-    x = (rng.standard_normal((1, 61, 83, 3)) * 50).astype(F)
+    rng = np.random.default_rng(k * 10 + stride + 100 * n)
+    x = (rng.standard_normal((n, 61, 83, 3)) * 50).astype(F)
     w = (rng.standard_normal((k, k, 3, cout)) * 0.01).astype(F)
-    if stride == 1:
-        conv = L.conv2d(x, w, 1, "SAME"); mode = "SAME"
-    else:
-        conv = L.conv2d_same(x, w, stride); mode = "EXPLICIT"
+    mode = "SAME" if stride == 1 else "EXPLICIT"
     if bn:
-        y, scale, shift = L.batch_norm(conv, rng.uniform(.5, 1.5, cout).astype(F), rng.standard_normal(cout).astype(F),
-                                       rng.standard_normal(cout).astype(F), rng.uniform(.5, 1.5, cout).astype(F), 1e-5)
+        _, scale, shift = L.batch_norm(np.zeros((1, 1, 1, cout), F), rng.uniform(.5, 1.5, cout).astype(F),
+                                       rng.standard_normal(cout).astype(F), rng.standard_normal(cout).astype(F),
+                                       rng.uniform(.5, 1.5, cout).astype(F), 1e-5)
     else:
         scale, shift = None, rng.standard_normal(cout).astype(F)
-        y = conv + shift
-    want = L.relu(y) if act == 1 else L.relu6(y)
     ho, wo, pt, pl = ops.conv_out_hw(61, 83, k, stride, mode)
-    out = torch.empty((1, ho, wo, cout), dtype=torch.float32, device="cuda")
-    ops.conv_first(dev(x), dev(w), None if scale is None else dev(scale), dev(shift), out, k, stride, pt, pl, act)
+    xd = dev(x)
+    buf, out = guarded_out((n, ho, wo, cout))
+    ops.conv_first(xd, dev(w), None if scale is None else dev(scale), dev(shift), out, k, stride, pt, pl, act)
     got = out.cpu().numpy()
-    assert got.shape == want.shape
-    assert np.abs(got - want).max() < 1e-4 * max(1.0, np.abs(want).max())
+    check_guarded(buf, out.numel())
+    assert np.array_equal(xd.cpu().numpy(), x)
+    r = check_fma_chain(got, x, w.transpose(3, 2, 0, 1), stride, pt, pl, ho, wo, k * k * 3, scale, shift, act)
+    print("\n[conv_first k=%d n=%d] max err / bound %.3f" % (k, n, r))
 
 
-@pytest.mark.parametrize("stride", [1, 2])
-def test_depthwise(cuda, stride):
+@pytest.mark.parametrize("stride,n", with_batch([1, 2]))
+def test_depthwise(cuda, stride, n):
     from tf_faster_rcnn_b200 import ops
-    rng = np.random.default_rng(stride)
+    rng = np.random.default_rng(stride + 10 * n)
     c = 64
-    x = rng.standard_normal((1, 37, 50, c)).astype(F)
+    x = rng.standard_normal((n, 37, 51, c)).astype(F)
     w = rng.standard_normal((3, 3, c, 1)).astype(F)
-    conv = L.conv2d_same(x, w, stride, groups=c)
-    y, scale, shift = L.batch_norm(conv, rng.uniform(.5, 1.5, c).astype(F), rng.standard_normal(c).astype(F),
+    _, scale, shift = L.batch_norm(np.zeros((1, 1, 1, c), F), rng.uniform(.5, 1.5, c).astype(F), rng.standard_normal(c).astype(F),
                                    rng.standard_normal(c).astype(F), rng.uniform(.5, 1.5, c).astype(F), 1e-3)
-    want = L.relu6(y)
-    ho, wo, pt, pl = ops.conv_out_hw(37, 50, 3, stride, "SAME" if stride == 1 else "EXPLICIT")
-    out = torch.empty((1, ho, wo, c), dtype=torch.float32, device="cuda")
-    ops.depthwise3x3(dev(x), dev(w.reshape(3, 3, c)), dev(scale), dev(shift), out, stride, pt, pl, 2)
+    ho, wo, pt, pl = ops.conv_out_hw(37, 51, 3, stride, "SAME" if stride == 1 else "EXPLICIT")
+    xd = dev(x)
+    buf, out = guarded_out((n, ho, wo, c))
+    ops.depthwise3x3(xd, dev(w.reshape(3, 3, c)), dev(scale), dev(shift), out, stride, pt, pl, 2)
     got = out.cpu().numpy()
-    assert got.shape == want.shape
-    assert np.abs(got - want).max() < 2e-5
+    check_guarded(buf, out.numel())
+    assert np.array_equal(xd.cpu().numpy(), x)
+    r = check_fma_chain(got, x, w.transpose(2, 3, 0, 1), stride, pt, pl, ho, wo, 9, scale, shift, 2, groups=c)
+    print("\n[depthwise s=%d n=%d] max err / bound %.3f" % (stride, n, r))
 
 
 def test_max_pools(cuda):

@@ -7,9 +7,11 @@
 //   FRCNN_CONV_F16X3 (default): x_hi = RN_f16(x), x_lo = RN_f16((x - x_hi) * 2^11).  fp16 has tf32's 11-bit significand, so
 //     every operand is carried to 2^-22 relative, with wgmma moving 16 k per instruction.  Range: the lo planes are pre-scaled
 //     by 2^11 (the cross terms are folded back with one fma by 2^-11), weights are pre-scaled per layer by a power of two so
-//     that max|w| sits in [2^13, 2^14) (undone exactly by `out_mult` in the epilogue), activations are converted with
-//     saturation (|x| <= 65504; anything the nets here produce is orders of magnitude below).
-//   FRCNN_CONV_TF32X3: the same split in tf32 (hi = RN_tf32(x), lo = RN_tf32(x - hi), no scaling), 8 k per instruction.
+//     that max|w| sits in [2^13, 2^14) (undone exactly by `out_mult` in the epilogue), activations are converted WITHOUT
+//     saturation: 2^-14 <= |x| < 65520 keeps 2^-22 relative (below 2^-14 the hi plane is subnormal and the loss grows to
+//     2^-12 at 2^-24); |x| >= 65520, +-Inf and NaN become Inf/NaN and so make the output non-finite, never finite and wrong.
+//   FRCNN_CONV_TF32X3: the same split in tf32 (hi = RN_tf32(x), lo = RN_tf32(x - hi), no scaling), 8 k per instruction;
+//     2^-22 relative from 2^-115 up to the tf32 overflow; non-finite inputs give non-finite outputs.
 //   FRCNN_CONV_F16X1 (throughput mode, NOT fp32-grade): the hi planes only, one product per pair.
 //
 // Data movement: activations stay plain NHWC fp32 in HBM.  For filter tap (r,s) the A operand of a tile of tn x th x tw
@@ -339,16 +341,19 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           if (T::TF32) {
             float x;
             asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x) : "r"(addr));
-            const float hi = to_tf32_fast(x);
+            // hi through cvt.rna: to_tf32_fast carries a NaN's high mantissa bits into the sign (0x7fffffff, the NaN the
+            // device's own arithmetic produces, becomes -0.0) and the NaN would vanish.  lo only needs the finite case: a
+            // non-finite x already makes hi non-finite.
+            const float hi = to_tf32(x);
             ahi[j][f] = __float_as_uint(hi);
             alo[j][f] = __float_as_uint(to_tf32_fast(__fsub_rn(x, hi)));
           } else {
             float2 x;
             asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(x.x), "=f"(x.y) : "r"(addr));
-            const uint32_t h = pack_f16x2_sat(x.x, x.y);
+            const uint32_t h = pack_f16x2_rn(x.x, x.y);
             const float2 fh = __half22float2(*reinterpret_cast<const __half2*>(&h));
             ahi[j][f] = h;
-            alo[j][f] = T::X1 ? 0u : pack_f16x2_sat(__fmul_rn(__fsub_rn(x.x, fh.x), 2048.f), __fmul_rn(__fsub_rn(x.y, fh.y), 2048.f));
+            alo[j][f] = T::X1 ? 0u : pack_f16x2_rn(__fmul_rn(__fsub_rn(x.x, fh.x), 2048.f), __fmul_rn(__fsub_rn(x.y, fh.y), 2048.f));
           }
         }
       }

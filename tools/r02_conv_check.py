@@ -3,6 +3,8 @@
     FRCNN_LIB_VARIANT=wd python tools/r02_conv_check.py [quick|full]
 
 With the watchdog library a barrier-protocol deadlock aborts the kernel and prints who waited on what instead of hanging.
+It prints numbers and asserts nothing.  Its range cases (tiny and large weights, the tf32 mode) are asserted element by
+element in tests/test_conv_gpu.py (weight channel spread, layer scale, activation scale sweep).
 """
 import ctypes as C
 import os
