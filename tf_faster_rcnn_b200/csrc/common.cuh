@@ -224,6 +224,18 @@ __device__ __forceinline__ float4 ld_nc_f4_pinned(const float* p) {
   asm volatile("ld.global.nc.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
   return v;
 }
+__device__ __forceinline__ float2 ld_nc_f2_pinned(const float* p) {
+  float2 v;
+  asm volatile("ld.global.nc.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "l"(p));
+  return v;
+}
+// the same, predicated: no memory access (and zeros) when `pred` is false
+__device__ __forceinline__ float2 ld_nc_f2_pinned_if(const float* p, bool pred) {
+  float2 v = make_float2(0.f, 0.f);
+  asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %3, 0;\n\t@q ld.global.nc.v2.f32 {%0, %1}, [%2];\n\t}\n"
+               : "+f"(v.x), "+f"(v.y) : "l"(p), "r"((int)pred));
+  return v;
+}
 __device__ __forceinline__ float ld_nc_f32_pinned(const float* p) {
   float v;
   asm volatile("ld.global.nc.f32 %0, [%1];" : "=f"(v) : "l"(p));

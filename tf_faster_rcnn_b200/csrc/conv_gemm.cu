@@ -146,26 +146,47 @@ __device__ __forceinline__ float2 finish2(const float2 v, const float2 sc, const
   return y;
 }
 
-// whole tile, cout % 4 == 0: float2 loads / stores (scale / shift are padded to the tile grid)
+// whole tile, cout % 4 == 0: float2 loads / stores (scale / shift are padded to the tile grid, so their loads need no bound).
+// The loads of a chunk of EPI_CHUNK column groups are all issued before the first of its stores: the per-group loop would
+// otherwise wait one full memory round trip (HBM for the residual) per 8 columns, BN / 8 times per tile, with the tensor
+// core idle.  Chunks bound the registers the in-flight loads hold (the partial registers are free here).
+constexpr int EPI_CHUNK = 8;
 template <int BN, bool RES, int ACT>
 __device__ __forceinline__ void epilogue_vec(const ConvKernelParams& p, const float (&acc)[BN / 2], const int cbase,
                                              const int pix0, const int pix1) {
   const int cout = p.cout;
+  constexpr int NJ = BN / 8;
+  constexpr int CH = NJ < EPI_CHUNK ? NJ : EPI_CHUNK;
+  static_assert(NJ % CH == 0, "chunking");
+  const float* const res0 = RES ? p.residual + (size_t)(pix0 >= 0 ? pix0 : 0) * cout : nullptr;
+  const float* const res1 = RES ? p.residual + (size_t)(pix1 >= 0 ? pix1 : 0) * cout : nullptr;
 #pragma unroll
-  for (int j = 0; j < BN / 8; ++j) {
-    const int c = cbase + 8 * j;
-    if (c >= cout) break;
-    const float2 sc = __ldg(reinterpret_cast<const float2*>(p.scale + c));
-    const float2 sh = __ldg(reinterpret_cast<const float2*>(p.shift + c));
-    if (pix0 >= 0) {
-      const size_t o = (size_t)pix0 * cout + c;
-      const float2 r = RES ? __ldg(reinterpret_cast<const float2*>(p.residual + o)) : sc;
-      *reinterpret_cast<float2*>(p.out + o) = finish2<RES, ACT>(make_float2(acc[4 * j], acc[4 * j + 1]), sc, sh, r);
+  for (int j0 = 0; j0 < NJ; j0 += CH) {
+    if (cbase + 8 * j0 >= cout) break;
+    float2 sc[CH], sh[CH], r0[CH], r1[CH];
+#pragma unroll
+    for (int jj = 0; jj < CH; ++jj) {
+      const int c = cbase + 8 * (j0 + jj);
+      sc[jj] = ld_nc_f2_pinned(p.scale + c);
+      sh[jj] = ld_nc_f2_pinned(p.shift + c);
+      if (RES) {
+        r0[jj] = ld_nc_f2_pinned_if(res0 + c, pix0 >= 0 && c < cout);
+        r1[jj] = ld_nc_f2_pinned_if(res1 + c, pix1 >= 0 && c < cout);
+      } else {
+        r0[jj] = r1[jj] = sc[jj];
+      }
     }
-    if (pix1 >= 0) {
-      const size_t o = (size_t)pix1 * cout + c;
-      const float2 r = RES ? __ldg(reinterpret_cast<const float2*>(p.residual + o)) : sc;
-      *reinterpret_cast<float2*>(p.out + o) = finish2<RES, ACT>(make_float2(acc[4 * j + 2], acc[4 * j + 3]), sc, sh, r);
+#pragma unroll
+    for (int jj = 0; jj < CH; ++jj) {
+      const int j = j0 + jj;
+      const int c = cbase + 8 * j;
+      if (c >= cout) break;
+      if (pix0 >= 0)
+        *reinterpret_cast<float2*>(p.out + (size_t)pix0 * cout + c) =
+            finish2<RES, ACT>(make_float2(acc[4 * j], acc[4 * j + 1]), sc[jj], sh[jj], r0[jj]);
+      if (pix1 >= 0)
+        *reinterpret_cast<float2*>(p.out + (size_t)pix1 * cout + c) =
+            finish2<RES, ACT>(make_float2(acc[4 * j + 2], acc[4 * j + 3]), sc[jj], sh[jj], r1[jj]);
     }
   }
 }
