@@ -223,6 +223,36 @@ int frcnn_detect_post(const float* cls_prob_dev, const float* pred_boxes_dev, co
                       int num_classes, float score_thresh, float nms_thresh, unsigned flags,
                       int max_per_image, int max_det, float* det_dev, int* ndet_dev, int record_stride, int* keep_dev,
                       int* keep_cnt_dev, float* keep_score_dev, void* workspace_dev, size_t workspace_bytes, void* stream);
+/* Soft-NMS (Bodla et al., ICCV 2017) in place of the greedy per-class NMS: an overlapping box has its score lowered instead of
+ * being dropped.  An extension beyond the reference (Detectron's TEST.SOFT_NMS).  Per candidate list a[0..N) (each row
+ * x1,y1,x2,y2,s):
+ *   for i = 0, 1, ... while i < N:
+ *     m = the lowest position in [i, N) holding the maximal score; swap a[i], a[m]; p = i + 1
+ *     while p < N: decay a[p] by a[i]; if a[p] overlapped a[i] and its new score < score_thresh: a[p] = a[N-1], N -= 1
+ *                  (position p is examined again) else p += 1
+ *   result: a[0..N) in this order with the decayed scores.
+ * Decay of b by t, every step a separate fp32 round-to-nearest operation, '+1' pixel areas:
+ *   iw = (min(t.x2,b.x2) - max(t.x1,b.x1)) + 1; if iw > 0: ih = (min(t.y2,b.y2) - max(t.y1,b.y1)) + 1; if ih > 0 they overlap:
+ *   ov = (iw*ih) / ((area(t) + area(b)) - iw*ih), area(u) = ((u.x2-u.x1)+1) * ((u.y2-u.y1)+1), and b.s = weight * b.s with
+ *   LINEAR: ov > nt ? 1 - ov : 1;  GAUSSIAN: RN_f32(exp_f64(-((ov*ov) / sigma)));  HARD: ov > nt ? 0 : 1.
+ * A box that does not overlap is neither decayed nor pruned.  Output scores never increase from row to row and, with
+ * score_thresh > 0, are > 0.  sigma > 0 and score_thresh > 0 are required (else FRCNN_ERR_ARG); capacity 8192 boxes. */
+#define FRCNN_SOFT_NMS_LINEAR 0
+#define FRCNN_SOFT_NMS_GAUSSIAN 1
+#define FRCNN_SOFT_NMS_HARD 2
+/* host buffers, synchronous, one set: the candidates are the n rows of dets_host [n, dim >= 5] in input order.  dets_out
+ * [n, 5] receives the kept rows in selection order with decayed scores, keep_out [n] their row indices in dets_host, num_out
+ * their count.  device_id < 0: the calling thread's current device; the caller's current device is left unchanged. */
+int frcnn_soft_nms_host(float* dets_out, int* keep_out, int* num_out, const float* dets_host, int n, int dim, int method,
+                        float sigma, float nt, float score_thresh, int device_id);
+/* frcnn_detect_post with Soft-NMS as the per-class stage: per class j >= 1 the candidates are the rows with score > score_thresh
+ * in ascending RoI order; keep / keep_cnt / keep_score hold the selection order and the decayed scores, and the max_per_image
+ * cap and records follow as in frcnn_detect_post.  prune_thresh is Soft-NMS's score_thresh above, nt the overlap threshold.
+ * workspace_dev is not used (the candidates fit in shared memory) and may be NULL. */
+int frcnn_detect_post_soft(const float* cls_prob_dev, const float* pred_boxes_dev, const int* num_rois_dev, int r, int batch,
+                           int num_classes, float score_thresh, int method, float sigma, float nt, float prune_thresh,
+                           int max_per_image, int max_det, float* det_dev, int* ndet_dev, int record_stride, int* keep_dev,
+                           int* keep_cnt_dev, float* keep_score_dev, void* workspace_dev, size_t workspace_bytes, void* stream);
 /* per-detection head features, run after frcnn_detect_post on the same keep_dev / keep_cnt_dev: slot k of image b is record
  * row k of that image (classes ascending, slot = prefix(keep_cnt)[c] + j, slot < max_det).  fc7_dev [batch*r, feat_dim] is the
  * head output the class / box FC read (feat_dim % 4 == 0, 16-byte aligned).  roi_out_dev int32 [batch, max_det] = RoI index

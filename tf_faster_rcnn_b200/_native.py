@@ -16,6 +16,7 @@ NMS_MODE_GPU_NMS = NMS_PLUS_ONE
 NMS_MODE_TF = NMS_SKIP_DEGENERATE
 ACT_NONE, ACT_RELU, ACT_RELU6 = 0, 1, 2
 CONV_F16X3, CONV_TF32X3, CONV_F16X1 = 0, 1, 2
+SOFT_NMS_METHODS = {"linear": 0, "gaussian": 1, "hard": 2}   # FRCNN_SOFT_NMS_*
 
 vp, ci, cf, cu, sz = C.c_void_p, C.c_int, C.c_float, C.c_uint, C.c_size_t
 ip, fp = C.POINTER(C.c_int), C.POINTER(C.c_float)
@@ -65,6 +66,8 @@ SIGNATURES = {
     "frcnn_bbox_decode": (ci, [vp, vp, ci, ci, ci, vp, vp, vp]),
     "frcnn_detect_post_workspace_bytes": (sz, [ci, ci, ci]),
     "frcnn_detect_post": (ci, [vp, vp, vp, ci, ci, ci, cf, cf, cu, ci, ci, vp, vp, ci, vp, vp, vp, vp, sz, vp]),
+    "frcnn_soft_nms_host": (ci, [fp, ip, ip, fp, ci, ci, ci, cf, cf, cf, ci]),
+    "frcnn_detect_post_soft": (ci, [vp, vp, vp, ci, ci, ci, cf, ci, cf, cf, cf, ci, ci, vp, vp, ci, vp, vp, vp, vp, sz, vp]),
     "frcnn_detect_features": (ci, [vp, vp, vp, ci, ci, ci, ci, ci, vp, vp, vp]),
     "frcnn_boxes_to_rois": (ci, [vp, vp, vp, ci, ci, vp, vp, vp]),
 }

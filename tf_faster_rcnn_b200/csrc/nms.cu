@@ -394,6 +394,231 @@ cap_emit_kernel(const float4* __restrict__ pred, int r, int C, int max_per_image
   }
 }
 
+// ---- Soft-NMS (Bodla et al., ICCV 2017) for the final per-class stage -----------------------------------------------
+// Sequential definition (include/frcnn_b200.h, frcnn_soft_nms_host): select the lowest position holding the maximal score,
+// swap it to the front, decay every later candidate by it, and replace each overlapped candidate that fell below the prune
+// threshold by the last one (the replacement is examined in turn).  The decays of one selection are independent of each other,
+// so one iteration is data parallel: decay everything, count the pruned positions, and fill the holes in closed form.  With
+// L = i+1, D = #pruned in [L, N) and B = N - D (the new count): survivors below B stay; the k-th pruned position below B
+// (ascending) receives the k-th survivor at or above B in DESCENDING position order -- exactly where the swap-with-last loop
+// puts it.  A survivor at p >= B knows its rank from the exclusive pruned count E(p): j = (N-1-p) - (D - E(p)).
+// Candidates live in shared memory as separate arrays (x1, y1, x2, y2, score, RoI index) plus the hole table; thread t owns
+// positions k*T + t.  Barriers per selection: the count, the hole table (only when something was pruned), the argmax.
+constexpr int SOFT_THREADS = 256, SOFT_PER = 4;            // r <= DET_CAP
+constexpr int SOFT_THREADS_BIG = 1024, SOFT_PER_BIG = 8;   // r <= DET_CAP_BIG
+static_assert(SOFT_THREADS * SOFT_PER == DET_CAP && SOFT_THREADS_BIG * SOFT_PER_BIG == DET_CAP_BIG, "soft-NMS capacities");
+
+struct SoftParams { int method; float sigma, nt, thresh; };
+
+constexpr size_t soft_smem_bytes(int cap) { return (size_t)cap * 24 + (size_t)(cap / 2) * 4; }   // at most cap/2 holes
+
+__device__ __forceinline__ float area_plus1(float x1, float y1, float x2, float y2) {
+  return __fmul_rn(__fadd_rn(__fsub_rn(x2, x1), 1.f), __fadd_rn(__fsub_rn(y2, y1), 1.f));
+}
+
+// Decays s by the selected box t (area ta).  Returns false (s untouched) when the boxes do not overlap.
+__device__ __forceinline__ bool soft_decay(float tx1, float ty1, float tx2, float ty2, float ta, float x1, float y1, float x2,
+                                           float y2, float& s, const SoftParams& p) {
+  const float iw = __fadd_rn(__fsub_rn(fminf(tx2, x2), fmaxf(tx1, x1)), 1.f);
+  if (!(iw > 0.f)) return false;
+  const float ih = __fadd_rn(__fsub_rn(fminf(ty2, y2), fmaxf(ty1, y1)), 1.f);
+  if (!(ih > 0.f)) return false;
+  const float inter = __fmul_rn(iw, ih);
+  const float ov = __fdiv_rn(inter, __fsub_rn(__fadd_rn(ta, area_plus1(x1, y1, x2, y2)), inter));
+  float w;
+  if (p.method == FRCNN_SOFT_NMS_GAUSSIAN) w = (float)exp(-(double)__fdiv_rn(__fmul_rn(ov, ov), p.sigma));   // exp_cr
+  else if (p.method == FRCNN_SOFT_NMS_LINEAR) w = ov > p.nt ? __fsub_rn(1.f, ov) : 1.f;
+  else w = ov > p.nt ? 0.f : 1.f;
+  s = __fmul_rn(w, s);
+  return true;
+}
+
+// Exclusive count of flag[k] over the positions k*T + tid of rows k < rows (rows is block uniform) into ex[k]; returns the
+// total.  One barrier; s_cnt [PER * T/32] is read after it, so the caller needs another barrier before the next call.
+template <int T, int PER>
+__device__ __forceinline__ int block_count_rows(const bool (&flag)[PER], int (&ex)[PER], int rows, int* s_cnt) {
+  constexpr int NW = T / 32;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = 0; k < PER; ++k) {
+    if (k < rows) {
+      const unsigned bal = __ballot_sync(0xffffffffu, flag[k]);
+      ex[k] = __popc(bal & ((1u << lane) - 1u));
+      if (lane == 0) s_cnt[k * NW + warp] = __popc(bal);
+    }
+  }
+  __syncthreads();
+  int run = 0;
+#pragma unroll
+  for (int k = 0; k < PER; ++k) {
+    if (k < rows) {
+      const int v = lane < NW ? s_cnt[k * NW + lane] : 0;
+      int inc = v;
+#pragma unroll
+      for (int o = 1; o < NW; o <<= 1) { const int u = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += u; }
+      ex[k] += run + __shfl_sync(0xffffffffu, inc - v, warp);
+      run += __shfl_sync(0xffffffffu, inc, NW - 1);
+    }
+  }
+  return run;
+}
+
+__device__ __forceinline__ void better_of(float& s, int& pos, float s2, int p2) {
+  if (s2 > s || (s2 == s && p2 < pos)) { s = s2; pos = p2; }
+}
+
+// Position of the block's best (score, position): larger score first, then lower position.  One barrier; every thread gets
+// the result.  Threads without a candidate pass (-inf, 0x7fffffff).
+template <int T>
+__device__ __forceinline__ int block_argmax(float s, int pos, float* s_as, int* s_ap) {
+  constexpr int NW = T / 32;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o; o >>= 1) better_of(s, pos, __shfl_xor_sync(0xffffffffu, s, o), __shfl_xor_sync(0xffffffffu, pos, o));
+  if (lane == 0) { s_as[warp] = s; s_ap[warp] = pos; }
+  __syncthreads();
+  s = lane < NW ? s_as[lane] : __int_as_float(0xff800000);
+  pos = lane < NW ? s_ap[lane] : 0x7fffffff;
+#pragma unroll
+  for (int o = 16; o; o >>= 1) better_of(s, pos, __shfl_xor_sync(0xffffffffu, s, o), __shfl_xor_sync(0xffffffffu, pos, o));
+  return pos;
+}
+
+// CTA-cooperative Soft-NMS over the inputs e < n for which is_cand(e) holds, taken in ascending e (blockDim.x == T).
+// box(e) / score(e) read an input; emit(i, e, box, score) is called by thread 0 for the i-th selection.  sm: dynamic shared
+// memory of soft_smem_bytes(T * PER).  Returns the number selected (block uniform).
+template <int T, int PER, typename CandFn, typename BoxFn, typename ScoreFn, typename EmitFn>
+__device__ int block_soft_nms(int n, CandFn is_cand, BoxFn box, ScoreFn score, const SoftParams prm, EmitFn emit, float* sm) {
+  constexpr int CAP = T * PER;
+  __shared__ int s_cnt[PER * (T / 32)];
+  __shared__ float s_as[T / 32];
+  __shared__ int s_ap[T / 32];
+  float* x1 = sm; float* y1 = sm + CAP; float* x2 = sm + 2 * CAP; float* y2 = sm + 3 * CAP; float* sc = sm + 4 * CAP;
+  int* id = reinterpret_cast<int*>(sm + 5 * CAP);
+  int* hole = id + CAP;
+  const int tid = threadIdx.x;
+  const float NEG_INF = __int_as_float(0xff800000);
+  bool f[PER];
+  int ex[PER];
+  // compaction of the candidates, ascending input index
+  int rows = (n + T - 1) / T;
+#pragma unroll
+  for (int k = 0; k < PER; ++k) { const int e = k * T + tid; f[k] = k < rows && e < n && is_cand(e); }
+  int N = block_count_rows<T, PER>(f, ex, rows, s_cnt);
+  float bs = NEG_INF;
+  int bp = 0x7fffffff;
+#pragma unroll
+  for (int k = 0; k < PER; ++k) {
+    if (f[k]) {
+      const int e = k * T + tid, p = ex[k];
+      const float4 b = box(e);
+      const float s = score(e);
+      x1[p] = b.x; y1[p] = b.y; x2[p] = b.z; y2[p] = b.w; sc[p] = s; id[p] = e;
+      better_of(bs, bp, s, p);
+    }
+  }
+  int m = block_argmax<T>(bs, bp, s_as, s_ap);
+  for (int i = 0; i < N; ++i) {
+    // the selection sits at m; position m holds the former a[i] (the swap is applied lazily: its owner reads from i).  Only
+    // NaN scores can leave the argmax empty; the sequential scan then keeps position i.
+    if (m >= N) m = i;
+    const float tx1 = x1[m], ty1 = y1[m], tx2 = x2[m], ty2 = y2[m];
+    if (tid == 0) emit(i, id[m], make_float4(tx1, ty1, tx2, ty2), sc[m]);
+    const float ta = area_plus1(tx1, ty1, tx2, ty2);
+    const int L = i + 1;
+    rows = (N + T - 1) / T;
+    float ns[PER];
+#pragma unroll
+    for (int k = 0; k < PER; ++k) {
+      const int p = k * T + tid;
+      f[k] = false; ns[k] = 0.f;
+      if (k < rows && p >= L && p < N) {
+        const int src = p == m ? i : p;
+        float s = sc[src];
+        const bool ov = soft_decay(tx1, ty1, tx2, ty2, ta, x1[src], y1[src], x2[src], y2[src], s, prm);
+        ns[k] = s;
+        f[k] = ov && s < prm.thresh;
+      }
+    }
+    const int D = block_count_rows<T, PER>(f, ex, rows, s_cnt);
+    const int B = N - D;
+    bs = NEG_INF; bp = 0x7fffffff;
+#pragma unroll
+    for (int k = 0; k < PER; ++k) {
+      const int p = k * T + tid;
+      if (k < rows && p >= L && p < B) {
+        if (f[k]) {
+          hole[ex[k]] = p;
+        } else {                                    // survivor that keeps its position
+          sc[p] = ns[k];
+          if (p == m && m != i) { x1[p] = x1[i]; y1[p] = y1[i]; x2[p] = x2[i]; y2[p] = y2[i]; id[p] = id[i]; }
+          better_of(bs, bp, ns[k], p);
+        }
+      }
+    }
+    if (D) {
+      __syncthreads();                              // hole table complete
+#pragma unroll
+      for (int k = 0; k < PER; ++k) {
+        const int p = k * T + tid;
+        if (k < rows && p >= B && p < N && !f[k]) {  // survivor above the new end: fills a hole
+          const int dst = hole[(N - 1 - p) - (D - ex[k])];
+          const int src = p == m ? i : p;
+          x1[dst] = x1[src]; y1[dst] = y1[src]; x2[dst] = x2[src]; y2[dst] = y2[src]; id[dst] = id[src]; sc[dst] = ns[k];
+          better_of(bs, bp, ns[k], dst);
+        }
+      }
+    }
+    N = B;
+    m = block_argmax<T>(bs, bp, s_as, s_ap);
+  }
+  return N;
+}
+
+// one CTA per (foreground class, image); the keep / keep_cnt / keep_score conventions of class_nms_kernel
+template <int T, int PER>
+__global__ void __launch_bounds__(T)
+class_soft_nms_kernel(const float* __restrict__ probs, const float4* __restrict__ pred, const int* __restrict__ num_rois, int r, int C,
+                      float score_thresh, SoftParams prm, int* __restrict__ keep, int* __restrict__ keep_cnt,
+                      float* __restrict__ keep_score) {
+  extern __shared__ __align__(16) float soft_dyn[];
+  const int cls = blockIdx.x + 1, img = blockIdx.y, tid = threadIdx.x;
+  probs += (size_t)img * r * C; pred += (size_t)img * r * C;
+  keep += (size_t)img * C * r; keep_score += (size_t)img * C * r; keep_cnt += (size_t)img * C;
+  const int nr = min(__ldg(num_rois + img), r);
+  int* ck = keep + (size_t)cls * r;
+  float* cs = keep_score + (size_t)cls * r;
+  const int nk = block_soft_nms<T, PER>(
+      nr, [&](int e) { return __ldg(probs + (size_t)e * C + cls) > score_thresh; },
+      [&](int e) { return __ldg(pred + (size_t)e * C + cls); }, [&](int e) { return __ldg(probs + (size_t)e * C + cls); }, prm,
+      [&](int i, int e, float4, float s) { ck[i] = e; cs[i] = s; }, soft_dyn);
+  for (int i = nk + tid; i < r; i += T) { ck[i] = -1; cs[i] = 0.f; }
+  if (tid == 0) keep_cnt[cls] = nk;
+  if (blockIdx.x == 0) {
+    for (int i = tid; i < r; i += T) { keep[i] = -1; keep_score[i] = 0.f; }
+    if (tid == 0) keep_cnt[0] = 0;
+  }
+}
+
+// one CTA: the whole input set (rows of `dim` floats: x1, y1, x2, y2, score, ...) is the candidate list
+template <int T, int PER>
+__global__ void __launch_bounds__(T)
+soft_nms_set_kernel(const float* __restrict__ dets, int n, int dim, SoftParams prm, float* __restrict__ dets_out,
+                    int* __restrict__ keep_out, int* __restrict__ num) {
+  extern __shared__ __align__(16) float soft_dyn[];
+  const int nk = block_soft_nms<T, PER>(
+      n, [](int) { return true; },
+      [&](int e) { const float* d = dets + (size_t)e * dim; return make_float4(d[0], d[1], d[2], d[3]); },
+      [&](int e) { return dets[(size_t)e * dim + 4]; }, prm,
+      [&](int i, int e, float4 b, float s) {
+        float* o = dets_out + (size_t)i * 5;
+        o[0] = b.x; o[1] = b.y; o[2] = b.z; o[3] = b.w; o[4] = s;
+        keep_out[i] = e;
+      },
+      soft_dyn);
+  if (threadIdx.x == 0) *num = nk;
+}
+
 // ---- per-detection head features ---------------------------------------------------------------------------
 // Runs after cap_emit_kernel and rebuilds its slot order from the truncated keep lists (classes ascending, slot =
 // prefix(keep_cnt)[c] + j), so slot k of the features is record row k.  One CTA per (block of FEAT_SLOTS slots, image):
@@ -569,6 +794,103 @@ extern "C" int frcnn_detect_post(const float* cls_prob, const float* pred_boxes,
                                                           keep, keep_cnt, keep_score, det, ndet,
                                                           record_stride ? record_stride : max_det * 6, record_stride ? record_stride : 1);
   FRCNN_LAUNCH_CHECK();
+  return OK;
+}
+
+static int soft_params(int method, float sigma, float nt, float score_thresh, SoftParams* p, const char* who) {
+  FRCNN_REQUIRE(method == FRCNN_SOFT_NMS_LINEAR || method == FRCNN_SOFT_NMS_GAUSSIAN || method == FRCNN_SOFT_NMS_HARD,
+                "%s: method %d is not FRCNN_SOFT_NMS_LINEAR / _GAUSSIAN / _HARD", who, method);
+  FRCNN_REQUIRE(sigma > 0.f, "%s: sigma must be > 0", who);
+  FRCNN_REQUIRE(score_thresh > 0.f, "%s: the prune threshold must be > 0", who);
+  FRCNN_REQUIRE(nt == nt, "%s: the overlap threshold is NaN", who);
+  *p = SoftParams{method, sigma, nt, score_thresh};
+  return OK;
+}
+
+// the big variant needs more than the default 48 KB of dynamic shared memory; set once per device
+template <typename K>
+static int soft_smem_attr(K kernel, bool (&done)[MAX_DEVICES]) {
+  int dev = 0;
+  FRCNN_CUDA(cudaGetDevice(&dev));
+  FRCNN_REQUIRE(dev >= 0 && dev < MAX_DEVICES, "device index %d out of range", dev);
+  if (!done[dev]) {
+    FRCNN_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)soft_smem_bytes(DET_CAP_BIG)));
+    done[dev] = true;
+  }
+  return OK;
+}
+
+extern "C" int frcnn_detect_post_soft(const float* cls_prob, const float* pred_boxes, const int* num_rois, int r, int batch,
+                                      int num_classes, float score_thresh, int method, float sigma, float nt, float prune_thresh,
+                                      int max_per_image, int max_det, float* det, int* ndet, int record_stride, int* keep,
+                                      int* keep_cnt, float* keep_score, void* workspace, size_t workspace_bytes, void* stream) {
+  (void)workspace; (void)workspace_bytes;
+  FRCNN_REQUIRE(cls_prob && pred_boxes && num_rois && det && ndet && keep && keep_cnt && keep_score, "detect_post_soft: null pointer");
+  FRCNN_REQUIRE(r > 0 && batch > 0 && num_classes >= 2 && num_classes <= 1024, "detect_post_soft: r>0, batch>0, 2<=C<=1024 required");
+  SoftParams prm;
+  int rc = soft_params(method, sigma, nt, prune_thresh, &prm, "detect_post_soft");
+  if (rc) return rc;
+  FRCNN_REQUIRE(record_stride == 0 || record_stride >= max_det * 6, "detect_post_soft: record_stride %d < max_det*6", record_stride);
+  if (r > DET_CAP_BIG) { set_error("detect_post_soft: %d RoIs per image > capacity %d", r, DET_CAP_BIG); return ERR_CAPACITY; }
+  cudaStream_t st = (cudaStream_t)stream;
+  const dim3 grid((unsigned)(num_classes - 1), (unsigned)batch);
+  const float4* pred = reinterpret_cast<const float4*>(pred_boxes);
+  if (r <= DET_CAP) {
+    class_soft_nms_kernel<SOFT_THREADS, SOFT_PER><<<grid, SOFT_THREADS, soft_smem_bytes(DET_CAP), st>>>(
+        cls_prob, pred, num_rois, r, num_classes, score_thresh, prm, keep, keep_cnt, keep_score);
+  } else {
+    static bool attr_done[MAX_DEVICES];
+    rc = soft_smem_attr(class_soft_nms_kernel<SOFT_THREADS_BIG, SOFT_PER_BIG>, attr_done);
+    if (rc) return rc;
+    class_soft_nms_kernel<SOFT_THREADS_BIG, SOFT_PER_BIG><<<grid, SOFT_THREADS_BIG, soft_smem_bytes(DET_CAP_BIG), st>>>(
+        cls_prob, pred, num_rois, r, num_classes, score_thresh, prm, keep, keep_cnt, keep_score);
+  }
+  FRCNN_LAUNCH_CHECK();
+  cap_emit_kernel<<<(unsigned)batch, NMS_THREADS, 0, st>>>(pred, r, num_classes, max_per_image, max_det, keep, keep_cnt, keep_score, det,
+                                                          ndet, record_stride ? record_stride : max_det * 6, record_stride ? record_stride : 1);
+  FRCNN_LAUNCH_CHECK();
+  return OK;
+}
+
+extern "C" int frcnn_soft_nms_host(float* dets_out, int* keep_out, int* num_out, const float* dets_host, int n, int dim, int method,
+                                   float sigma, float nt, float score_thresh, int device_id) {
+  FRCNN_REQUIRE(dets_out && keep_out && num_out, "soft_nms_host: null output");
+  *num_out = 0;
+  SoftParams prm;
+  int rc = soft_params(method, sigma, nt, score_thresh, &prm, "soft_nms_host");
+  if (rc) return rc;
+  if (n <= 0) return OK;
+  FRCNN_REQUIRE(dets_host && dim >= 5, "soft_nms_host: bad input (rows of >= 5 floats: x1, y1, x2, y2, score)");
+  if (n > DET_CAP_BIG) { set_error("soft_nms_host: %d boxes > capacity %d", n, DET_CAP_BIG); return ERR_CAPACITY; }
+  int cur = -1;
+  FRCNN_CUDA(cudaGetDevice(&cur));
+  const int dev = device_id < 0 ? cur : device_id;
+  if (cur != dev) FRCNN_CUDA(cudaSetDevice(dev));
+  static bool attr_done[MAX_DEVICES];
+  if (n > DET_CAP) rc = soft_smem_attr(soft_nms_set_kernel<SOFT_THREADS_BIG, SOFT_PER_BIG>, attr_done);
+  float* din = nullptr; float* dout = nullptr; int* dkeep = nullptr;
+  cudaError_t e = cudaSuccess;
+  if (!rc) {
+    e = cudaMalloc(&din, (size_t)n * dim * sizeof(float));
+    if (e == cudaSuccess) e = cudaMalloc(&dout, (size_t)n * 5 * sizeof(float));
+    if (e == cudaSuccess) e = cudaMalloc(&dkeep, (size_t)(n + 1) * sizeof(int));
+    if (e == cudaSuccess) e = cudaMemcpy(din, dets_host, (size_t)n * dim * sizeof(float), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) {
+      if (n <= DET_CAP)
+        soft_nms_set_kernel<SOFT_THREADS, SOFT_PER><<<1, SOFT_THREADS, soft_smem_bytes(DET_CAP)>>>(din, n, dim, prm, dout, dkeep, dkeep + n);
+      else
+        soft_nms_set_kernel<SOFT_THREADS_BIG, SOFT_PER_BIG><<<1, SOFT_THREADS_BIG, soft_smem_bytes(DET_CAP_BIG)>>>(din, n, dim, prm, dout,
+                                                                                                                 dkeep, dkeep + n);
+      e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpy(num_out, dkeep + n, sizeof(int), cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && *num_out > 0) e = cudaMemcpy(keep_out, dkeep, (size_t)(*num_out) * sizeof(int), cudaMemcpyDeviceToHost);
+    if (e == cudaSuccess && *num_out > 0) e = cudaMemcpy(dets_out, dout, (size_t)(*num_out) * 5 * sizeof(float), cudaMemcpyDeviceToHost);
+    cudaFree(din); cudaFree(dout); cudaFree(dkeep);
+  }
+  if (cur != dev) cudaSetDevice(cur);                    // leave the caller's (torch's) current device untouched
+  if (rc) return rc;
+  if (e != cudaSuccess) { *num_out = 0; return cuda_fail(e, "frcnn_soft_nms_host", __FILE__, __LINE__); }
   return OK;
 }
 

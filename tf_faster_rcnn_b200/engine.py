@@ -363,10 +363,12 @@ class ShapePlan:
         self.feat_out = self.roi_out = self.features_step = None
 
     def _ensure_post(self, features=False):
-        """(Re)build the detection-record buffers and the post step for the current score / NMS thresholds and cap; with
-        `features`, also the per-detection feature buffers and their gather step."""
+        """(Re)build the detection-record buffers and the post step for the current score / NMS thresholds, cap and Soft-NMS
+        setting; with `features`, also the per-detection feature buffers and their gather step."""
         o = self.net.options
-        key = (float(o["score_thresh"]), float(o["nms_thresh"]), bool(o["use_gpu_nms"]), int(o["max_per_image"]))
+        soft = o.get("soft_nms")
+        key = (float(o["score_thresh"]), float(o["nms_thresh"]), bool(o["use_gpu_nms"]), int(o["max_per_image"]),
+               None if soft is None else soft_nms_args(*soft))
         if key != self.post_key:
             self._build_post(key)
         if features and self.features_step is None:
@@ -386,9 +388,17 @@ class ShapePlan:
         self.max_det = 2 * mpi + 56 if mpi > 0 else R * (C - 1)
         stride = REC_HEADER + self.max_det * 6
         thr, flags = nms_threshold(key[1], key[2])
+        soft = key[4]
 
         def make_post(rec):
             def post():
+                if soft is not None:
+                    N.check(N.lib().frcnn_detect_post_soft(ops._p(self.cls_prob), ops._p(self.pred_boxes), ops._p(self.num_rois), R, B, C,
+                                                           key[0], soft[0], soft[1], float(F(key[1])), soft[2], mpi, self.max_det,
+                                                           C_void(rec.data_ptr() + 4 * REC_HEADER), ops._p(rec), stride,
+                                                           ops._p(self.keep), ops._p(self.keep_cnt), ops._p(self.keep_score), None, 0,
+                                                           ops._stream()), "detect_post_soft")
+                    return
                 N.check(N.lib().frcnn_detect_post(ops._p(self.cls_prob), ops._p(self.pred_boxes), ops._p(self.num_rois), R, B, C, key[0],
                                                   thr, flags, mpi, self.max_det, C_void(rec.data_ptr() + 4 * REC_HEADER), ops._p(rec), stride,
                                                   ops._p(self.keep), ops._p(self.keep_cnt), ops._p(self.keep_score), ops._p(self.post_ws),
@@ -505,6 +515,26 @@ def check_feature_mode(max_per_image):
     if max_per_image <= 0:
         raise ValueError("per-detection features need max_per_image > 0: without the cap the record buffer holds every "
                          "(RoI, class) pair, R*(C-1) feature rows per image (hundreds of MB)")
+
+
+def soft_nms_args(method, sigma, score_thresh):
+    """Soft-NMS parameters -> (FRCNN_SOFT_NMS_* code, fp32 sigma, fp32 prune threshold); raises ValueError before any device work."""
+    if method not in N.SOFT_NMS_METHODS:
+        raise ValueError("Soft-NMS METHOD %r: expected one of %s" % (method, ", ".join(sorted(N.SOFT_NMS_METHODS))))
+    s32, t32 = F(sigma), F(score_thresh)
+    if not s32 > 0:
+        raise ValueError("Soft-NMS SIGMA must be > 0, got %r" % (sigma,))
+    if not t32 > 0:
+        raise ValueError("Soft-NMS SCORE_THRESH must be > 0 (the record cap assumes positive scores), got %r" % (score_thresh,))
+    return N.SOFT_NMS_METHODS[method], float(s32), float(t32)
+
+
+def soft_nms_option(node):
+    """cfg.TEST.SOFT_NMS -> the network option: None when disabled, else the checked (METHOD, SIGMA, SCORE_THRESH)."""
+    if not node["ENABLED"]:
+        return None
+    soft_nms_args(node["METHOD"], node["SIGMA"], node["SCORE_THRESH"])
+    return (node["METHOD"], float(node["SIGMA"]), float(node["SCORE_THRESH"]))
 
 
 def nms_threshold(thresh, use_gpu_nms):

@@ -53,6 +53,9 @@ cfg = AttrDict(
     TEST=dict(
         SCALES=(600,), MAX_SIZE=1000, NMS=0.3, SVM=False, BBOX_REG=True, HAS_RPN=False, PROPOSAL_METHOD="gt",
         RPN_NMS_THRESH=0.7, RPN_PRE_NMS_TOP_N=6000, RPN_POST_NMS_TOP_N=300, MODE="nms", RPN_TOP_N=5000,
+        # extension (Detectron's TEST.SOFT_NMS): Soft-NMS in place of the final per-class NMS; overlap threshold TEST.NMS.
+        # METHOD linear | gaussian | hard, SIGMA > 0 (gaussian), SCORE_THRESH > 0 (prune threshold); USE_GPU_NMS does not apply
+        SOFT_NMS=dict(ENABLED=False, METHOD="linear", SIGMA=0.5, SCORE_THRESH=0.001),
     ),
     RESNET=dict(MAX_POOL=False, FIXED_BLOCKS=1),
     MOBILENET=dict(REGU_DEPTH=False, FIXED_LAYERS=5, WEIGHT_DECAY=0.00004, DEPTH_MULTIPLIER=1.0),

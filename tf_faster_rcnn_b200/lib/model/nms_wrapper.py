@@ -4,7 +4,9 @@ empty input -> []; otherwise indices into the UNSORTED `dets`, in descending-sco
 Both of the reference's predicates run on the GPU here (there is no CPU implementation):
   cfg.USE_GPU_NMS and not force_cpu -> gpu_nms semantics ('+1' areas, suppress when IoU >  thresh)
   otherwise                         -> cpu_nms semantics ('+1' areas, suppress when ovr >= thresh)
-The host argsort mirrors gpu_nms.pyx:25-28 / cpu_nms.pyx:25 but is stable (ties: lower index first)."""
+The host argsort mirrors gpu_nms.pyx:25-28 / cpu_nms.pyx:25 but is stable (ties: lower index first).
+
+`soft_nms(...)` is an extension beyond the reference with Detectron's contract (Soft-NMS, Bodla et al. 2017), also on the GPU."""
 import numpy as np
 
 from model.config import cfg
@@ -19,3 +21,14 @@ def nms(dets, thresh, force_cpu=False):
     t32, flags = engine.nms_threshold(thresh, bool(cfg.USE_GPU_NMS) and not force_cpu)
     keep = ops.nms_host(dets[order], t32, flags, device_id=-1)   # the process's current device (rank-local under torchrun)
     return list(order[keep])
+
+
+def soft_nms(dets, sigma=0.5, overlap_thresh=0.3, score_thresh=0.001, method="linear"):
+    """Soft-NMS of dets [n, 5] (x1, y1, x2, y2, score), taken in row order, semantics of include/frcnn_b200.h
+    (frcnn_soft_nms_host).  method: 'linear' | 'gaussian' | 'hard'; every parameter is used as fp32.
+    -> (dets_out [k, 5] fp32 in selection order with the decayed scores, keep [k] indices into dets).  Empty input ->
+    (zeros((0, 5)), [])."""
+    code, sigma32, thresh32 = engine.soft_nms_args(method, sigma, score_thresh)
+    if dets.shape[0] == 0:
+        return np.zeros((0, 5), np.float32), []
+    return ops.soft_nms_host(dets, code, sigma32, float(np.float32(overlap_thresh)), thresh32, device_id=-1)

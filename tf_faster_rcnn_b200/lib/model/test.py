@@ -17,7 +17,8 @@ import numpy as np
 import torch
 
 from model.config import cfg, get_output_dir
-from model.nms_wrapper import nms
+from model.nms_wrapper import nms, soft_nms
+from tf_faster_rcnn_b200 import engine
 from utils.blob import im_list_to_blob
 from utils.timer import Timer
 
@@ -124,11 +125,16 @@ def apply_nms(all_boxes, thresh):
 
 
 def _detections_python_loop(scores, boxes, num_classes, thresh, max_per_image):
-    """test.py:162-180 verbatim flow over the (GPU) nms()."""
+    """test.py:162-180 verbatim flow over the (GPU) nms(), or soft_nms() per class when TEST.SOFT_NMS.ENABLED."""
     per_class = [np.zeros((0, 5), np.float32)]
     for j in range(1, num_classes):
         inds = np.where(scores[:, j] > thresh)[0]
         cls_dets = np.hstack((boxes[inds, j * 4:(j + 1) * 4], scores[inds, j][:, np.newaxis])).astype(np.float32, copy=False)
+        if cfg.TEST.SOFT_NMS.ENABLED:
+            sn = cfg.TEST.SOFT_NMS
+            kept, _ = soft_nms(cls_dets, sn.SIGMA, cfg.TEST.NMS, sn.SCORE_THRESH, sn.METHOD)
+            per_class.append(kept)
+            continue
         keep = nms(cls_dets, cfg.TEST.NMS)
         per_class.append(cls_dets[keep, :])
     if max_per_image > 0:
@@ -154,6 +160,7 @@ def detect_image(net, im, thresh=0., max_per_image=100):
 def _set_post_options(net, thresh, max_per_image):
     net.options["score_thresh"], net.options["max_per_image"] = float(thresh), int(max_per_image)
     net.options["nms_thresh"] = cfg.TEST.NMS
+    net.options["soft_nms"] = engine.soft_nms_option(cfg.TEST.SOFT_NMS)
 
 
 def _detect_record(net, im, thresh, max_per_image):

@@ -229,6 +229,16 @@ def detect_post(cls_prob, pred_boxes, num_rois, num_classes, score_thresh, nms_t
                                       _stream()), "detect_post")
 
 
+def detect_post_soft(cls_prob, pred_boxes, num_rois, num_classes, score_thresh, method, sigma, nt, prune_thresh, max_per_image, det,
+                     ndet, keep, keep_cnt, keep_score, batch=1):
+    """detect_post with Soft-NMS as the per-class stage; method is an FRCNN_SOFT_NMS_* code (N.SOFT_NMS_METHODS)."""
+    r = cls_prob.shape[0] // batch
+    max_det = det.shape[-2]
+    N.check(N.lib().frcnn_detect_post_soft(_p(cls_prob), _p(pred_boxes), _p(num_rois), r, batch, num_classes, float(score_thresh),
+                                           int(method), float(sigma), float(nt), float(prune_thresh), max_per_image, max_det, _p(det),
+                                           _p(ndet), 0, _p(keep), _p(keep_cnt), _p(keep_score), None, 0, _stream()), "detect_post_soft")
+
+
 def detect_features(keep, keep_cnt, fc7, num_classes, feat_out, roi_out):
     """After detect_post: keep [batch, C, r], keep_cnt [batch, C] (the capped lists), fc7 [batch*r, F] ->
     feat_out [batch, max_det, F] = fc7 row of record slot k, roi_out int32 [batch, max_det] (-1 past the count)."""
@@ -259,3 +269,17 @@ def nms_host(sorted_dets, thresh, flags, device_id=-1):
     N.check(N.lib().frcnn_nms_host(keep.ctypes.data_as(N.ip), C.byref(num), d.ctypes.data_as(N.fp), n, d.shape[1] if n else 5,
                                    float(thresh), device_id, flags), "nms_host")
     return keep[:num.value].copy()
+
+
+def soft_nms_host(dets, method, sigma, nt, score_thresh, device_id=-1):
+    """Soft-NMS of one set of HOST rows [n, >=5] (x1, y1, x2, y2, score, ...), candidates in row order; method is an
+    FRCNN_SOFT_NMS_* code.  -> (rows [k,5] fp32 in selection order with decayed scores, keep [k] int32 rows of dets)."""
+    d = np.ascontiguousarray(dets, dtype=np.float32)
+    n = d.shape[0]
+    out = np.empty((max(n, 1), 5), dtype=np.float32)
+    keep = np.empty(max(n, 1), dtype=np.int32)
+    num = C.c_int(0)
+    N.check(N.lib().frcnn_soft_nms_host(out.ctypes.data_as(N.fp), keep.ctypes.data_as(N.ip), C.byref(num), d.ctypes.data_as(N.fp), n,
+                                        d.shape[1] if n else 5, int(method), float(sigma), float(nt), float(score_thresh), device_id),
+            "soft_nms_host")
+    return out[:num.value].copy(), keep[:num.value].copy()
