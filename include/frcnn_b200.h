@@ -168,6 +168,10 @@ int frcnn_spatial_mean(const float* in_dev, float* out_dev, int r, int hw, int c
  * H = cvRound(h0*fy), W = cvRound(w0*fx) computed by the caller.  means3 is a HOST pointer. */
 int frcnn_preprocess(const unsigned char* img_dev, int h0, int w0, const double* means3, double fx, double fy,
                      float* blob_dev, int H, int W, void* stream);
+/* the same blob of the mirrored image img[:, ::-1] (the flipped view of test-time augmentation): mirror first, then resize, so
+ * that un-flipping a box is exact in original pixels.  Bit for bit frcnn_preprocess of a host-mirrored image. */
+int frcnn_preprocess_hflip(const unsigned char* img_dev, int h0, int w0, const double* means3, double fx, double fy,
+                           float* blob_dev, int H, int W, void* stream);
 
 /* ---- (4) proposal / detection stages.  Every stage takes `batch` images of one blob shape (the reference is batch 1,
  * lib/nets/network.py:388; batch > 1 is the throughput extension of SURVEY.md 8(f) rank 4): per-image arrays are
@@ -266,6 +270,26 @@ int frcnn_detect_features(const int* keep_dev, const int* keep_cnt_dev, const fl
  * [batch] = min(count, cap).  No clipping: crop_and_resize samples outside the feature map as 0. */
 int frcnn_boxes_to_rois(const float* boxes_dev, const int* counts_dev, const float* im_meta_dev, int batch, int cap,
                         float* rois_dev, int* num_rois_dev, void* stream);
+
+/* ---- test-time augmentation (Detectron's TEST.BBOX_AUG, union mode) -- an extension beyond the reference ----
+ * A view is a pair (scale, flip): the base view (TEST.SCALES[0], TEST.MAX_SIZE), one view per TEST.BBOX_AUG.SCALES entry
+ * (capped by TEST.BBOX_AUG.MAX_SIZE, the resize rule of _get_image_blob), and with H_FLIP the mirrored twin of each.  A mirrored
+ * view is the blob of img[:, ::-1] (frcnn_preprocess_hflip).  Each view runs the unchanged network and im_detect tail
+ * (frcnn_bbox_decode, one-sided clip); frcnn_aug_union then merges the views, and the unchanged frcnn_detect_post /
+ * frcnn_detect_post_soft run on the union (r = R_union = sum of the views' rows, <= 8192).
+ * Union of image b, in view order (the caller's order; the Python layer uses Detectron's: flipped base, then each extra scale
+ * followed by its flip, the base view last), the valid rows [0, n_v) of view v with n_v = clamp(num_rois_v[b], 0, R_v):
+ *   union row off_v + i = view row i (i < n_v), off_v = n_0 + ... + n_{v-1}; rows past the total are zero;
+ *   cls_prob copied; pred_boxes copied, and for a mirrored view un-flipped with W = orig_w of im_meta_dev[b] (fp32, two
+ *   roundings each): x1 = (W - x2') - 1, x2 = (W - x1') - 1, y unchanged;  num_rois_dev[b] = sum of n_v.
+ * Host arrays of num_views (<= FRCNN_AUG_MAX_VIEWS) entries: the views' device pointers cls_prob [batch, R_v, C], pred_boxes
+ * [batch, R_v, 4C] (16-byte aligned), num_rois int32 [batch]; rois_per_view R_v > 0; flip_views 0 / 1.  im_meta_dev [batch, 3] as
+ * for frcnn_bbox_decode.  Outputs: cls_prob_dev [batch, R_union, C], pred_boxes_dev [batch, R_union, 4C], num_rois_dev int32
+ * [batch].  The pointers are copied into the kernel's parameters, so the launch is CUDA-graph capturable. */
+#define FRCNN_AUG_MAX_VIEWS 16
+int frcnn_aug_union(const float* const* cls_prob_views, const float* const* pred_boxes_views, const int* const* num_rois_views,
+                    const int* rois_per_view, const int* flip_views, int num_views, int batch, int num_classes,
+                    const float* im_meta_dev, float* cls_prob_dev, float* pred_boxes_dev, int* num_rois_dev, void* stream);
 
 #ifdef __cplusplus
 }

@@ -17,6 +17,7 @@ NMS_MODE_TF = NMS_SKIP_DEGENERATE
 ACT_NONE, ACT_RELU, ACT_RELU6 = 0, 1, 2
 CONV_F16X3, CONV_TF32X3, CONV_F16X1 = 0, 1, 2
 SOFT_NMS_METHODS = {"linear": 0, "gaussian": 1, "hard": 2}   # FRCNN_SOFT_NMS_*
+AUG_MAX_VIEWS = 16                                            # FRCNN_AUG_MAX_VIEWS
 
 vp, ci, cf, cu, sz = C.c_void_p, C.c_int, C.c_float, C.c_uint, C.c_size_t
 ip, fp = C.POINTER(C.c_int), C.POINTER(C.c_float)
@@ -70,6 +71,8 @@ SIGNATURES = {
     "frcnn_detect_post_soft": (ci, [vp, vp, vp, ci, ci, ci, cf, ci, cf, cf, cf, ci, ci, vp, vp, ci, vp, vp, vp, vp, sz, vp]),
     "frcnn_detect_features": (ci, [vp, vp, vp, ci, ci, ci, ci, ci, vp, vp, vp]),
     "frcnn_boxes_to_rois": (ci, [vp, vp, vp, ci, ci, vp, vp, vp]),
+    "frcnn_preprocess_hflip": (ci, [vp, ci, ci, C.POINTER(C.c_double), C.c_double, C.c_double, vp, ci, ci, vp]),
+    "frcnn_aug_union": (ci, [C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), ip, ip, ci, ci, ci, vp, vp, vp, vp, vp]),
 }
 
 _lib = None

@@ -402,10 +402,65 @@ __global__ void boxes_to_rois_kernel(const float4* __restrict__ boxes, const int
   }
 }
 
+// ---- test-time augmentation: the union of the views' im_detect outputs, ahead of the per-class NMS ------------------------
+// The per-view pointers travel inside the kernel's parameter block (__grid_constant__: indexed in place, no local copy), so
+// one captured launch serves every call of the same views.
+struct AugViews {
+  const float* prob[FRCNN_AUG_MAX_VIEWS];    // [batch, rows, C] of the view
+  const float4* box[FRCNN_AUG_MAX_VIEWS];    // [batch, rows, C] float4 (x1, y1, x2, y2)
+  const int* num[FRCNN_AUG_MAX_VIEWS];       // [batch] valid-row counts
+  int rows[FRCNN_AUG_MAX_VIEWS];
+  int flip[FRCNN_AUG_MAX_VIEWS];
+};
+
+// Thread per (union row, class) of image blockIdx.y; every union row is written exactly once.  View v's valid rows [0, n_v)
+// land at [off_v, off_v + n_v), off_v = n_0 + ... + n_{v-1}; the rows past the total are zero.  A mirrored view's boxes are
+// un-flipped in original pixels: x1 = (W - x2') - 1, x2 = (W - x1') - 1, two fp32 roundings each, W = im_meta's orig_w.
+__global__ void __launch_bounds__(256)
+aug_union_kernel(const __grid_constant__ AugViews vw, int nv, int C, int ru, const float* __restrict__ im_meta,
+                 float* __restrict__ prob, float4* __restrict__ box, int* __restrict__ num) {
+  __shared__ int s_off[FRCNN_AUG_MAX_VIEWS + 1];
+  const int b = blockIdx.y;
+  if (threadIdx.x == 0) {
+    int o = 0;
+    for (int v = 0; v < nv; ++v) {
+      s_off[v] = o;
+      o += min(max(__ldg(vw.num[v] + b), 0), vw.rows[v]);
+    }
+    s_off[nv] = o;
+    if (blockIdx.x == 0) num[b] = o;
+  }
+  __syncthreads();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= ru * C) return;
+  const int u = i / C, c = i - u * C;
+  const size_t dst = ((size_t)b * ru + u) * C + c;
+  if (u >= s_off[nv]) {
+    prob[dst] = 0.f;
+    box[dst] = make_float4(0.f, 0.f, 0.f, 0.f);
+    return;
+  }
+  int v = 0;
+  while (u >= s_off[v + 1]) ++v;                       // terminates: u < s_off[nv]; views with no rows are stepped over
+  const size_t src = ((size_t)b * vw.rows[v] + (u - s_off[v])) * C + c;
+  prob[dst] = __ldg(vw.prob[v] + src);
+  float4 q = __ldg(vw.box[v] + src);
+  if (vw.flip[v]) {
+    const float w = __ldg(im_meta + b * 3 + 2);
+    const float x1 = __fsub_rn(__fsub_rn(w, q.z), 1.f), x2 = __fsub_rn(__fsub_rn(w, q.x), 1.f);
+    q.x = x1;
+    q.z = x2;
+  }
+  box[dst] = q;
+}
+
 // ---- image -> blob on the device (SURVEY 8(f) rank 2): mean subtraction + cv2.resize(INTER_LINEAR) restated ----------
 // lib/model/test.py:35-36 (float32(pixel) - PIXEL_MEANS, evaluated in double and rounded once, as numpy's in-place
 // float32 -= float64 does) followed by OpenCV's float bilinear resize: source coordinate (dx + 0.5) / fx - 0.5 in double,
 // floor + fraction in double, clamp; horizontal pass then vertical pass.
+// HFLIP: the blob of the mirrored image img[:, ::-1] (test-time augmentation): the same arithmetic on the mirrored source
+// grid, whose column sx is the image's column w0 - 1 - sx.
+template <bool HFLIP>
 __global__ void preprocess_kernel(const unsigned char* __restrict__ img, int h0, int w0, double m0, double m1, double m2,
                                   double inv_fx, double inv_fy, float* __restrict__ blob, int H, int W) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -423,14 +478,15 @@ __global__ void preprocess_kernel(const unsigned char* __restrict__ img, int h0,
   if (sy < 0) { fy = 0.f; sy = 0; }
   if (sy >= h0 - 1) { fy = 0.f; sy = h0 - 1; }
   const int sx1 = min(sx + 1, w0 - 1), sy1 = min(sy + 1, h0 - 1);
+  const int ix0 = HFLIP ? w0 - 1 - sx : sx, ix1 = HFLIP ? w0 - 1 - sx1 : sx1;
   const float a0 = 1.f - fx, a1 = fx, b0 = 1.f - fy, b1 = fy;
   const double mean[3] = {m0, m1, m2};
   const unsigned char* r0 = img + (size_t)sy * w0 * 3;
   const unsigned char* r1 = img + (size_t)sy1 * w0 * 3;
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
-    const float v00 = (float)((double)r0[sx * 3 + c] - mean[c]), v01 = (float)((double)r0[sx1 * 3 + c] - mean[c]);
-    const float v10 = (float)((double)r1[sx * 3 + c] - mean[c]), v11 = (float)((double)r1[sx1 * 3 + c] - mean[c]);
+    const float v00 = (float)((double)r0[ix0 * 3 + c] - mean[c]), v01 = (float)((double)r0[ix1 * 3 + c] - mean[c]);
+    const float v10 = (float)((double)r1[ix0 * 3 + c] - mean[c]), v11 = (float)((double)r1[ix1 * 3 + c] - mean[c]);
     const float t0 = __fadd_rn(__fmul_rn(v00, a0), __fmul_rn(v01, a1));
     const float t1 = __fadd_rn(__fmul_rn(v10, a0), __fmul_rn(v11, a1));
     blob[(size_t)i * 3 + c] = __fadd_rn(__fmul_rn(t0, b0), __fmul_rn(t1, b1));
@@ -570,11 +626,51 @@ extern "C" int frcnn_boxes_to_rois(const float* boxes, const int* counts, const 
   return OK;
 }
 
+template <bool HFLIP>
+static int preprocess(const unsigned char* img_dev, int h0, int w0, const double* means3, double fx, double fy, float* blob_dev, int H,
+                      int W, void* stream) {
+  FRCNN_REQUIRE(img_dev && means3 && blob_dev && h0 > 0 && w0 > 0 && H > 0 && W > 0 && fx > 0 && fy > 0, "preprocess: bad argument");
+  preprocess_kernel<HFLIP><<<blocks_for((long)H * W, 256), 256, 0, (cudaStream_t)stream>>>(img_dev, h0, w0, means3[0], means3[1], means3[2],
+                                                                                         1.0 / fx, 1.0 / fy, blob_dev, H, W);
+  FRCNN_LAUNCH_CHECK();
+  return OK;
+}
+
 extern "C" int frcnn_preprocess(const unsigned char* img_dev, int h0, int w0, const double* means3, double fx, double fy,
                                 float* blob_dev, int H, int W, void* stream) {
-  FRCNN_REQUIRE(img_dev && means3 && blob_dev && h0 > 0 && w0 > 0 && H > 0 && W > 0 && fx > 0 && fy > 0, "preprocess: bad argument");
-  preprocess_kernel<<<blocks_for((long)H * W, 256), 256, 0, (cudaStream_t)stream>>>(img_dev, h0, w0, means3[0], means3[1], means3[2],
-                                                                                  1.0 / fx, 1.0 / fy, blob_dev, H, W);
+  return preprocess<false>(img_dev, h0, w0, means3, fx, fy, blob_dev, H, W, stream);
+}
+
+extern "C" int frcnn_preprocess_hflip(const unsigned char* img_dev, int h0, int w0, const double* means3, double fx, double fy,
+                                      float* blob_dev, int H, int W, void* stream) {
+  return preprocess<true>(img_dev, h0, w0, means3, fx, fy, blob_dev, H, W, stream);
+}
+
+extern "C" int frcnn_aug_union(const float* const* cls_prob_views, const float* const* pred_boxes_views, const int* const* num_rois_views,
+                               const int* rois_per_view, const int* flip_views, int num_views, int batch, int num_classes,
+                               const float* im_meta_dev, float* cls_prob_dev, float* pred_boxes_dev, int* num_rois_dev, void* stream) {
+  FRCNN_REQUIRE(cls_prob_views && pred_boxes_views && num_rois_views && rois_per_view && flip_views && im_meta_dev && cls_prob_dev &&
+                    pred_boxes_dev && num_rois_dev, "aug_union: null pointer");
+  FRCNN_REQUIRE(num_views > 0 && batch > 0 && num_classes > 0, "aug_union: num_views>0, batch>0, num_classes>0 required");
+  if (num_views > FRCNN_AUG_MAX_VIEWS) { set_error("aug_union: %d views > capacity %d", num_views, FRCNN_AUG_MAX_VIEWS); return ERR_CAPACITY; }
+  FRCNN_REQUIRE(((uintptr_t)pred_boxes_dev & 15) == 0, "aug_union: pred_boxes_dev must be 16-byte aligned");
+  AugViews vw = {};
+  long ru = 0;
+  for (int v = 0; v < num_views; ++v) {
+    FRCNN_REQUIRE(cls_prob_views[v] && pred_boxes_views[v] && num_rois_views[v], "aug_union: null pointer of view %d", v);
+    FRCNN_REQUIRE(((uintptr_t)pred_boxes_views[v] & 15) == 0, "aug_union: pred_boxes of view %d must be 16-byte aligned", v);
+    FRCNN_REQUIRE(rois_per_view[v] > 0 && (flip_views[v] == 0 || flip_views[v] == 1), "aug_union: view %d: rows > 0, flip 0 or 1 required", v);
+    vw.prob[v] = cls_prob_views[v];
+    vw.box[v] = reinterpret_cast<const float4*>(pred_boxes_views[v]);
+    vw.num[v] = num_rois_views[v];
+    vw.rows[v] = rois_per_view[v];
+    vw.flip[v] = flip_views[v];
+    ru += rois_per_view[v];
+  }
+  FRCNN_REQUIRE(ru * num_classes < (1l << 31), "aug_union: %ld union rows x %d classes too large", ru, num_classes);
+  const dim3 grid(blocks_for(ru * num_classes, 256), (unsigned)batch);
+  aug_union_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(vw, num_views, num_classes, (int)ru, im_meta_dev, cls_prob_dev,
+                                                           reinterpret_cast<float4*>(pred_boxes_dev), num_rois_dev);
   FRCNN_LAUNCH_CHECK();
   return OK;
 }

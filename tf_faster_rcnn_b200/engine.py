@@ -472,6 +472,158 @@ class ShapePlan:
         return split_host_records(self.rec.cpu(), self.max_det)
 
 
+AUG_MAX_ROIS = 8192    # RoI rows per image that frcnn_detect_post / _soft take: the cap of the union
+
+
+class AugPlan:
+    """Test-time augmentation (TEST.BBOX_AUG) for `batch` images whose views have the blob shapes `views` = ((h, w, flip), ...),
+    in union order.  Views of one blob shape share one ShapePlan at batch k*batch from the network's plan cache: unflipped views
+    take the first slots, so an identity view and its flip are slots [0, B) and [B, 2B) of a batch-2B plan.  One call replays
+    the sub-plans' im_detect graphs, then frcnn_aug_union merges the views' rows into the union buffers and the post step runs
+    on them.  The union, the post step and its two alternating record buffers are this object's; the post step is ShapePlan's
+    own construction (the methods below are ShapePlan's), run on R = the sum of the views' rows."""
+
+    _ensure_post = ShapePlan._ensure_post
+    _build_post = ShapePlan._build_post
+    _select = ShapePlan._select
+    records = ShapePlan.records
+
+    def __init__(self, net, views, batch):
+        self.net, self.views, self.batch = net, tuple(views), int(batch)
+        B, C = self.batch, net.num_classes
+        self.shapes, self.view_slot, counts = aug_groups(self.views)
+        self.group_batch = {hw: k * B for hw, k in counts.items()}
+        self.subs = {}
+        self.graphs = {}
+        self.use_graph = net.use_cuda_graph
+        self.bind()
+        self.rows = [self.subs[(h, w)].R for h, w, _ in self.views]
+        R = self.R = sum(self.rows)
+        self.cls_prob = ops.zeros((B * R, C)); self.pred_boxes = ops.zeros((B * R, 4 * C))
+        self.num_rois = ops.zeros((B,), dtype=torch.int32)
+        self.keep = ops.zeros((B, C, R), dtype=torch.int32); self.keep_cnt = ops.zeros((B, C), dtype=torch.int32)
+        self.keep_score = ops.zeros((B, C, R))
+        self.post_ws = ops.detect_post_workspace(R, C, B)
+        self.post_key = None
+        self.recs = [None, None]
+        self.rec = self.det = self.ndet = None
+        self.post_steps = [None, None]
+        self.feat_out = self.roi_out = self.features_step = None
+        self.double_buffer = False
+        self.slot = 0
+        self.max_det = 0
+
+    def bind(self):
+        """Fetch the sub-plans from the network's plan cache (marking them recently used).  A plan evicted by the LRU and rebuilt
+        is a new object with new buffers: then the union's pointer table is rebuilt and the captured union / post graphs are
+        dropped."""
+        changed = False
+        for hw in self.shapes:
+            p = self.net.plan_for(hw[0], hw[1], self.group_batch[hw])
+            if self.subs.get(hw) is not p:
+                self.subs[hw] = p
+                changed = True
+        if changed:
+            B, C = self.batch, self.net.num_classes
+            table = []
+            for v, (h, w, flip) in enumerate(self.views):
+                p, k = self.subs[(h, w)], self.view_slot[v] * B
+                table.append((p.cls_prob.data_ptr() + 4 * k * p.R * C, p.pred_boxes.data_ptr() + 16 * k * p.R * C,
+                              p.num_rois.data_ptr() + 4 * k, p.R, flip))
+            p0 = self.subs[self.views[0][:2]]
+            self.table, self.meta_ptr = table, p0.im_meta.data_ptr() + 12 * self.view_slot[0] * B
+            self.graphs.clear()
+
+    def view_image(self, v):
+        """View v's input slice [batch, h, w, 3] of its sub-plan's image buffer (fill it, then launch)."""
+        B, k = self.batch, self.view_slot[v]
+        return self.subs[self.views[v][:2]].image[k * B:(k + 1) * B]
+
+    def _union(self):
+        ops.aug_union(self.table, self.net.num_classes, self.meta_ptr, self.cls_prob, self.pred_boxes, self.num_rois)
+
+    def launch(self, scales, orig_hws, detect=True):
+        """Enqueue one call (inputs already in view_image(v)).  scales[v][b]: view v's scale factor of image b; orig_hws: per
+        image (h, w).  detect=False stops after the union (im_detect's outputs in cls_prob / pred_boxes / num_rois)."""
+        B = self.batch
+        metas = {hw: [None] * p.batch for hw, p in self.subs.items()}
+        for v, (h, w, _) in enumerate(self.views):
+            k = self.view_slot[v] * B
+            for b in range(B):
+                metas[(h, w)][k + b] = (float(scales[v][b]), int(orig_hws[b][0]), int(orig_hws[b][1]))
+        for hw, p in self.subs.items():
+            p.launch(post=True, meta=metas[hw])
+        if not detect:
+            self._union()
+            return
+        self._ensure_post()
+        self._select(self.slot ^ 1 if self.double_buffer else 0)
+        fns = [self._union, self.post_steps[self.slot]]
+        if not self.use_graph:
+            for fn in fns:
+                fn()
+            return
+        g = self.graphs.get(("detect", self.slot))
+        if g is None:
+            for fn in fns:
+                fn()
+            torch.cuda.current_stream().synchronize()
+            g = self.graphs[("detect", self.slot)] = LaunchGraph(fns)
+        g.replay()
+
+
+def aug_groups(views):
+    """views ((h, w, flip), ...) -> (distinct (h, w) in first-use order, slot of each view within its shape's plan, views per
+    shape).  Unflipped views take the lower slots, then flipped ones, each in view order."""
+    shapes, counts, slot = [], {}, [0] * len(views)
+    for h, w, _ in views:
+        if (h, w) not in shapes:
+            shapes.append((h, w))
+    for v in sorted(range(len(views)), key=lambda v: (bool(views[v][2]), v)):
+        hw = tuple(views[v][:2])
+        slot[v] = counts.get(hw, 0)
+        counts[hw] = slot[v] + 1
+    return shapes, slot, counts
+
+
+def aug_rois_per_view(options):
+    """RoI rows per image of one view: what ShapePlan._rpn_rois allots (RPN_TOP_N in 'top' mode, else RPN_POST_NMS_TOP_N)."""
+    return int(options["rpn_top_n"] if options["test_mode"] == "top" else options["rpn_post_nms_top_n"])
+
+
+def check_aug_views(views, rois_per_view, max_plans):
+    """views: ((h, w, flip), ...) of one call; raises ValueError before any device work."""
+    nv = len(views)
+    if not 0 < nv <= N.AUG_MAX_VIEWS:
+        raise ValueError("test-time augmentation with %d views: 1 to %d are supported" % (nv, N.AUG_MAX_VIEWS))
+    if nv * rois_per_view > AUG_MAX_ROIS:
+        raise ValueError("test-time augmentation: %d views x %d RoIs = %d union rows per image, more than the %d the per-class NMS "
+                         "takes (fewer views, or fewer RoIs per view)" % (nv, rois_per_view, nv * rois_per_view, AUG_MAX_ROIS))
+    shapes = len(set((int(h), int(w)) for h, w, _ in views))
+    if shapes > max_plans:
+        raise ValueError("test-time augmentation: the views have %d distinct blob shapes but the plan cache holds %d "
+                         "(Network.MAX_PLANS); the plans of one call would evict each other" % (shapes, max_plans))
+
+
+def bbox_aug_option(node, bbox_reg=True):
+    """cfg.TEST.BBOX_AUG -> None when disabled, else the checked (H_FLIP, SCALES, MAX_SIZE); raises ValueError before any device
+    work.  The view count is (1 + len(SCALES)) * (2 if H_FLIP else 1)."""
+    if not node["ENABLED"]:
+        return None
+    if not bbox_reg:
+        raise ValueError("TEST.BBOX_AUG needs TEST.BBOX_REG = True: the union merges the views' regressed boxes")
+    scales = tuple(node["SCALES"])
+    for s in scales:
+        if not s > 0:
+            raise ValueError("TEST.BBOX_AUG.SCALES must be positive short sides, got %r" % (scales,))
+    if not node["MAX_SIZE"] > 0:
+        raise ValueError("TEST.BBOX_AUG.MAX_SIZE must be positive, got %r" % (node["MAX_SIZE"],))
+    nv = (1 + len(scales)) * (2 if node["H_FLIP"] else 1)
+    if nv > N.AUG_MAX_VIEWS:
+        raise ValueError("TEST.BBOX_AUG gives %d views: at most %d are supported" % (nv, N.AUG_MAX_VIEWS))
+    return bool(node["H_FLIP"]), scales, node["MAX_SIZE"]
+
+
 def split_host_records(host, max_det):
     """host: CPU float32 tensor [B, REC_HEADER + max_det*6] -> list of [n,6] numpy arrays; raises when a record set did not fit."""
     counts = host.view(torch.int32)[:, 0].numpy()

@@ -56,6 +56,10 @@ cfg = AttrDict(
         # extension (Detectron's TEST.SOFT_NMS): Soft-NMS in place of the final per-class NMS; overlap threshold TEST.NMS.
         # METHOD linear | gaussian | hard, SIGMA > 0 (gaussian), SCORE_THRESH > 0 (prune threshold); USE_GPU_NMS does not apply
         SOFT_NMS=dict(ENABLED=False, METHOD="linear", SIGMA=0.5, SCORE_THRESH=0.001),
+        # extension (Detectron's TEST.BBOX_AUG, union mode): test-time augmentation.  Views: the base (SCALES[0], MAX_SIZE), one per
+        # BBOX_AUG.SCALES entry (short side, long side capped by BBOX_AUG.MAX_SIZE), and with H_FLIP the mirrored twin of each; the
+        # boxes of every view are merged ahead of the per-class NMS (model/test.py::aug_views gives the order)
+        BBOX_AUG=dict(ENABLED=False, H_FLIP=False, SCALES=(), MAX_SIZE=2000),
     ),
     RESNET=dict(MAX_POOL=False, FIXED_BLOCKS=1),
     MOBILENET=dict(REGU_DEPTH=False, FIXED_LAYERS=5, WEIGHT_DECAY=0.00004, DEPTH_MULTIPLIER=1.0),

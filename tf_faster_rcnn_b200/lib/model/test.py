@@ -37,25 +37,93 @@ def _get_image_blob(im):
     TEST.SCALES[i] unless that would push the long side over TEST.MAX_SIZE."""
     pixels = im.astype(np.float32, copy=True)
     pixels -= cfg.PIXEL_MEANS
-    short_side, long_side = min(pixels.shape[:2]), max(pixels.shape[:2])
     resized, factors = [], []
     for target in cfg.TEST.SCALES:
-        f = float(target) / float(short_side)
-        if np.round(f * long_side) > cfg.TEST.MAX_SIZE:
-            f = float(cfg.TEST.MAX_SIZE) / float(long_side)
-        resized.append(cv2.resize(pixels, None, None, fx=f, fy=f, interpolation=cv2.INTER_LINEAR))
+        r, f = _resize(pixels, target, cfg.TEST.MAX_SIZE)
+        resized.append(r)
         factors.append(f)
     return im_list_to_blob(resized), np.array(factors)
 
 
-def blob_geometry(im_shape):
-    """(H, W, scale) of the blob _get_image_blob would build for an image of this shape (first TEST scale)."""
+def _scale_factor(im_shape, target, max_size):
+    """short side -> target unless the long side would exceed max_size"""
     short_side, long_side = min(im_shape[:2]), max(im_shape[:2])
-    f = float(cfg.TEST.SCALES[0]) / float(short_side)
-    if np.round(f * long_side) > cfg.TEST.MAX_SIZE:
-        f = float(cfg.TEST.MAX_SIZE) / float(long_side)
+    f = float(target) / float(short_side)
+    if np.round(f * long_side) > max_size:
+        f = float(max_size) / float(long_side)
+    return f
+
+
+def _resize(pixels, target, max_size):
+    f = _scale_factor(pixels.shape, target, max_size)
+    return cv2.resize(pixels, None, None, fx=f, fy=f, interpolation=cv2.INTER_LINEAR), f
+
+
+def blob_geometry(im_shape, target=None, max_size=None):
+    """(H, W, scale) of the blob _get_image_blob would build for an image of this shape (first TEST scale, or `target` short
+    side capped by `max_size`)."""
+    f = _scale_factor(im_shape, cfg.TEST.SCALES[0] if target is None else target, cfg.TEST.MAX_SIZE if max_size is None else max_size)
     # cv2.resize with fx/fy: dsize = cvRound(size * f) (round half to even)
     return int(np.rint(im_shape[0] * f)), int(np.rint(im_shape[1] * f)), f
+
+
+# ---- test-time augmentation (TEST.BBOX_AUG; Detectron's im_detect_bbox_aug in union mode) ---------------------------------------
+# A view is (scale, flip): the base view (TEST.SCALES[0], TEST.MAX_SIZE), one view per BBOX_AUG.SCALES entry (that short side,
+# the long side capped by BBOX_AUG.MAX_SIZE) and, with H_FLIP, the mirrored twin of each.  A mirrored view is resize(im[:, ::-1]):
+# mirrored first, then resized, so un-flipping its boxes (x1 = (W - x2') - 1, x2 = (W - x1') - 1 in fp32, W the original width)
+# is exact in original pixels.  The union of an image takes the valid RoI rows of each view in Detectron's order: the flipped
+# base view, then every extra scale followed by its flip, the base view last.  The order decides only ties and Soft-NMS's
+# candidate order.  The per-class NMS (greedy or Soft-NMS), the max_per_image cap and the records then run unchanged on the union.
+
+def aug_views(im_shape):
+    """The views of an image of this shape in union order: [(target, max_size, flip), ...]."""
+    flip, scales, max_size = engine.bbox_aug_option(cfg.TEST.BBOX_AUG, cfg.TEST.BBOX_REG)
+    base = (cfg.TEST.SCALES[0], cfg.TEST.MAX_SIZE)
+    views = [base + (True,)] if flip else []
+    for s in scales:
+        views.append((s, max_size, False))
+        if flip:
+            views.append((s, max_size, True))
+    return views + [base + (False,)]
+
+
+def aug_view_blob(im, target, max_size, flip):
+    """One view's host blob ([1,H,W,3] fp32, scale factor): _get_image_blob's arithmetic on im, or on im[:, ::-1] when flipped."""
+    pixels = (im[:, ::-1] if flip else im).astype(np.float32, copy=True)
+    pixels -= cfg.PIXEL_MEANS
+    r, f = _resize(pixels, target, max_size)
+    return im_list_to_blob([r]), f
+
+
+def _run_aug(net, ims, detect, double_buffer=False, device_preprocess=False):
+    """ims: images whose views have the same blob shapes -> the AugPlan after one launch (records when `detect`, else the union
+    left in its cls_prob / pred_boxes / num_rois).  Every check raises before device work."""
+    views = aug_views(ims[0].shape)
+    hws = [im.shape[:2] for im in ims]
+    if device_preprocess:
+        geo = [blob_geometry(ims[0].shape, t, m) for t, m, _ in views]
+        aug = net.aug_plan([(g[0], g[1], fl) for g, (_, _, fl) in zip(geo, views)], len(ims))
+        means = np.asarray(cfg.PIXEL_MEANS, dtype=np.float64).ravel()
+        from tf_faster_rcnn_b200 import ops
+        for b, im in enumerate(ims):
+            img = torch.from_numpy(np.ascontiguousarray(im)).cuda(non_blocking=True)
+            for v, (_, _, fl) in enumerate(views):
+                ops.preprocess(img, means, geo[v][2], geo[v][2], aug.view_image(v)[b:b + 1], hflip=fl)
+        scales = [[g[2]] * len(ims) for g in geo]
+    else:
+        per_view = [[aug_view_blob(im, *view) for im in ims] for view in views]
+        aug = net.aug_plan([(pv[0][0].shape[1], pv[0][0].shape[2], fl) for pv, (_, _, fl) in zip(per_view, views)], len(ims))
+        for v, pv in enumerate(per_view):
+            aug.view_image(v).copy_(torch.from_numpy(np.concatenate([x[0] for x in pv], axis=0)), non_blocking=True)
+        scales = [[x[1] for x in pv] for pv in per_view]
+    aug.double_buffer = double_buffer
+    aug.launch(scales, hws, detect=detect)
+    return aug
+
+
+def _aug_key(im):
+    """The tuple of view blob shapes of an image: images with equal keys share one augmented launch."""
+    return tuple(blob_geometry(im.shape, t, m)[:2] + (fl,) for t, m, fl in aug_views(im.shape))
 
 
 def _run_device_preprocess(net, im, post, detect, boxes=None):
@@ -80,7 +148,14 @@ def _get_blobs(im):
 def im_detect(sess, net, im, boxes=None):
     """-> scores [R, C] fp32, pred_boxes [R, 4C] fp32 in ORIGINAL-image pixels.  boxes: [n, 4] boxes (x1,y1,x2,y2,
     original-image pixels) scored instead of the RPN's proposals (Fast R-CNN, TEST.HAS_RPN = False): then R = n, in the
-    given order."""
+    given order.  With TEST.BBOX_AUG.ENABLED: the union of the views (R = its row count, see aug_views)."""
+    if cfg.TEST.BBOX_AUG.ENABLED:
+        if boxes is not None:
+            raise ValueError("TEST.BBOX_AUG (test-time augmentation) does not apply to caller boxes: disable it for this call")
+        aug = _run_aug(net, [im], detect=False, device_preprocess=DEVICE_PREPROCESS)
+        torch.cuda.current_stream().synchronize()
+        r = int(aug.num_rois[0].item())
+        return aug.cls_prob[:r].cpu().numpy(), aug.pred_boxes[:r].cpu().numpy()
     if boxes is not None:
         from tf_faster_rcnn_b200 import engine
         boxes = engine.check_boxes([np.asarray(boxes, dtype=np.float32)], 1)[0]
@@ -147,11 +222,14 @@ def _detections_python_loop(scores, boxes, num_classes, thresh, max_per_image):
 
 def detect_image(net, im, thresh=0., max_per_image=100):
     """One image through the fused device path -> list over classes of fp32 [k,5] (x1,y1,x2,y2,score)."""
-    blobs, im_scales = _get_blobs(im)
-    blob = blobs['data']
-    im_info = np.array([blob.shape[1], blob.shape[2], im_scales[0]], dtype=np.float32)
     _set_post_options(net, thresh, max_per_image)
-    det, _ = net.detect(blob, im_info, im.shape[:2])
+    if cfg.TEST.BBOX_AUG.ENABLED:
+        det = _run_aug(net, [im], detect=True).records()[0]
+    else:
+        blobs, im_scales = _get_blobs(im)
+        blob = blobs['data']
+        im_info = np.array([blob.shape[1], blob.shape[2], im_scales[0]], dtype=np.float32)
+        det, _ = net.detect(blob, im_info, im.shape[:2])
     C = net.num_classes
     cls = det[:, 5].astype(np.int64)
     return [det[cls == j, :5] for j in range(C)]
@@ -166,7 +244,11 @@ def _set_post_options(net, thresh, max_per_image):
 def _detect_record(net, im, thresh, max_per_image):
     """Fused path for one image, result left on the device: the plan's record buffer of this launch
     ([REC_HEADER + max_det*6] fp32, int32 count in word 0), stream-ordered.  Consecutive launches of a plan alternate between
-    two record buffers, so the record stays valid while the NEXT image runs (the sharded loop gathers it meanwhile)."""
+    two record buffers, so the record stays valid while the NEXT image runs (the sharded loop gathers it meanwhile); so do the
+    augmented launches of TEST.BBOX_AUG."""
+    if cfg.TEST.BBOX_AUG.ENABLED:
+        _set_post_options(net, thresh, max_per_image)
+        return _run_aug(net, [im], detect=True, double_buffer=True).rec[0]
     blobs, im_scales = _get_blobs(im)
     blob = blobs['data']
     im_info = np.array([blob.shape[1], blob.shape[2], im_scales[0]], dtype=np.float32)
@@ -184,6 +266,18 @@ def detect_images(net, ims, thresh=0., max_per_image=100, batch_size=None):
     bs = int(batch_size or BATCH_SIZE)
     _set_post_options(net, thresh, max_per_image)
     C = net.num_classes
+    if cfg.TEST.BBOX_AUG.ENABLED:      # groups: consecutive images whose whole tuple of view blob shapes matches
+        out, i = [], 0
+        keys = [_aug_key(im) for im in ims]
+        while i < len(ims):
+            j = i + 1
+            while j < len(ims) and j - i < bs and keys[j] == keys[i]:
+                j += 1
+            for det in _run_aug(net, ims[i:j], detect=True).records():
+                cls = det[:, 5].astype(np.int64)
+                out.append([det[cls == c, :5] for c in range(C)])
+            i = j
+        return out
     prepared = []
     for im in ims:
         blobs, im_scales = _get_blobs(im)

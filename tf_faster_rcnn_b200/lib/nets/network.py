@@ -16,6 +16,11 @@ from tf_faster_rcnn_b200 import engine, _native
 _REGISTRY = []   # networks created in this process (the tensorflow shim's Saver.restore walks it)
 
 
+def _no_bbox_aug(what):
+    if cfg.TEST.BBOX_AUG.ENABLED:
+        raise ValueError("TEST.BBOX_AUG (test-time augmentation) does not apply to %s: disable it for this call" % what)
+
+
 class Network(object):
     def __init__(self):
         self._feat_stride = [16, ]
@@ -24,6 +29,7 @@ class Network(object):
         self._scope = None
         self.weights = None
         self._plans = {}
+        self._aug_plans = {}   # test-time augmentation: (views, batch) -> engine.AugPlan over plans of _plans
         self.use_cuda_graph = True
         _REGISTRY.append(self)
 
@@ -53,6 +59,7 @@ class Network(object):
         if self.options["test_mode"] not in ("nms", "top"):
             raise NotImplementedError
         self._plans = {}
+        self._aug_plans = {}
         return {"rois": None}
 
     def test_image(self, sess, image, im_info):
@@ -114,6 +121,7 @@ class Network(object):
                                  % (self.arch_name(), self._num_classes, self._num_anchors, "\n  ".join(problems)))
         self.weights = engine.Weights(dict(tensors))
         self._plans = {}
+        self._aug_plans = {}
 
     MAX_PLANS = int(os.environ.get("FRCNN_MAX_PLANS", "6"))
 
@@ -138,6 +146,37 @@ class Network(object):
                                     rois_source="rpn" if cap is None else "boxes", cap=cap)
         self._plans[key] = plan                             # most recently used last
         return plan
+
+    def aug_plan(self, views, batch):
+        """AugPlan of test-time augmentation for `batch` images with views ((h, w, flip), ...) in union order; its sub-plans come
+        from plan_for.  Raises ValueError (too many views, union rows or blob shapes) before any device work."""
+        views = tuple((int(h), int(w), bool(f)) for h, w, f in views)
+        engine.check_aug_views(views, engine.aug_rois_per_view(self.options), max(1, self.MAX_PLANS))
+        key = (views, int(batch))
+        aug = self._aug_plans.pop(key, None)
+        if aug is None:
+            while len(self._aug_plans) >= max(1, self.MAX_PLANS):
+                self._aug_plans.pop(next(iter(self._aug_plans)))
+            aug = engine.AugPlan(self, views, int(batch))
+        else:
+            aug.bind()
+        self._aug_plans[key] = aug                          # most recently used last
+        return aug
+
+    def detect_aug(self, blobs, im_scales, orig_hws, flips):
+        """Test-time augmentation (TEST.BBOX_AUG) through the fused device path: per view v a blob blobs[v] [B, H_v, W_v, 3]
+        (numpy or torch; a mirrored view is the blob of the mirrored image), im_scales[v] its B scale factors and flips[v];
+        orig_hws: per image the original (h, w).  The views' detections are merged in the given order ahead of the per-class
+        NMS and the max_per_image cap.  -> (list of B det arrays [n,6], aug plan)."""
+        b = int(blobs[0].shape[0])
+        assert len(blobs) == len(im_scales) == len(flips) and len(orig_hws) == b
+        aug = self.aug_plan([(x.shape[1], x.shape[2], f) for x, f in zip(blobs, flips)], b)
+        for v, x in enumerate(blobs):
+            assert x.shape[0] == b and x.shape[3] == 3
+            src = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32))
+            aug.view_image(v).copy_(src, non_blocking=True)
+        aug.launch(im_scales, orig_hws, detect=True)
+        return aug.records(), aug
 
     def _copy_in(self, plan, image):
         if isinstance(image, torch.Tensor):
@@ -177,6 +216,7 @@ class Network(object):
         Needs options['max_per_image'] > 0."""
         b = int(images.shape[0])
         assert images.shape[3] == 3 and len(im_scales) == b and len(orig_hws) == b
+        _no_bbox_aug("per-detection features (detect_features)")
         engine.check_feature_mode(int(self.options["max_per_image"]))
         plan = self.plan_for(images.shape[1], images.shape[2], b)
         self._copy_in(plan, images)
@@ -189,6 +229,7 @@ class Network(object):
         """Enqueue `images` [B,H,W,3] with caller boxes as the RoIs on a caller-box plan (no sync) -> plan."""
         b = int(images.shape[0])
         assert images.shape[3] == 3 and len(im_scales) == b and len(orig_hws) == b
+        _no_bbox_aug("caller boxes (score_boxes / im_detect(boxes=))")
         boxes = engine.check_boxes(boxes, b)
         plan = self.plan_for(images.shape[1], images.shape[2], b, cap=engine.box_capacity(max(a.shape[0] for a in boxes)))
         self._copy_in(plan, images)

@@ -152,13 +152,16 @@ def spatial_mean(x, out):
     N.check(N.lib().frcnn_spatial_mean(_p(_f32(x)), _p(_f32(out)), r, hw, c, _stream()), "spatial_mean")
 
 
-def preprocess(img_u8_dev, means3, fx, fy, blob):
-    """uint8 BGR [h0,w0,3] (device) -> mean-subtracted, bilinearly resized fp32 blob [1,H,W,3] (device)."""
+def preprocess(img_u8_dev, means3, fx, fy, blob, hflip=False):
+    """uint8 BGR [h0,w0,3] (device) -> mean-subtracted, bilinearly resized fp32 blob [1,H,W,3] (device).  hflip: the blob of the
+    mirrored image img[:, ::-1] (test-time augmentation's flipped view)."""
     h0, w0, _ = img_u8_dev.shape
     _, H, W, _ = blob.shape
+    assert blob.is_contiguous()
     m = (C.c_double * 3)(*[float(v) for v in means3])
-    N.check(N.lib().frcnn_preprocess(C.c_void_p(img_u8_dev.data_ptr()), h0, w0, m, float(fx), float(fy), _p(blob), H, W, _stream()),
-            "preprocess")
+    fn = N.lib().frcnn_preprocess_hflip if hflip else N.lib().frcnn_preprocess
+    N.check(fn(C.c_void_p(img_u8_dev.data_ptr()), h0, w0, m, float(fx), float(fy), _p(blob), H, W, _stream()),
+            "preprocess_hflip" if hflip else "preprocess")
 
 
 def rpn_decode(rpn_out, delta_col, base_anchors, num_anchors, fh, fw, im_h, im_w, scores, props, feat_stride=16, batch=1):
@@ -253,6 +256,19 @@ def boxes_to_rois(boxes, counts, im_meta, rois, num_rois):
     batch, cap, _ = boxes.shape
     N.check(N.lib().frcnn_boxes_to_rois(_p(_f32(boxes)), _p(counts), _p(_f32(im_meta)), batch, cap, _p(_f32(rois)), _p(num_rois),
                                         _stream()), "boxes_to_rois")
+
+
+def aug_union(views, num_classes, im_meta, cls_prob, pred_boxes, num_rois):
+    """Test-time augmentation union.  views: per view (cls_prob, pred_boxes, num_rois, rows, flip) with the three as device
+    addresses (ints) of the view's [batch, rows, C] / [batch, rows, 4C] / int32 [batch]; im_meta: device address of [batch, 3]
+    (orig_w in column 2).  cls_prob [batch, R_union, C], pred_boxes [batch, R_union, 4C], num_rois int32 [batch] (tensors)."""
+    nv = len(views)
+    ptrs = [(C.c_void_p * nv)(*[v[k] for v in views]) for k in range(3)]
+    rows = (C.c_int * nv)(*[int(v[3]) for v in views])
+    flips = (C.c_int * nv)(*[int(bool(v[4])) for v in views])
+    batch = num_rois.shape[0]
+    N.check(N.lib().frcnn_aug_union(ptrs[0], ptrs[1], ptrs[2], rows, flips, nv, batch, num_classes, C.c_void_p(im_meta), _p(_f32(cls_prob)),
+                                    _p(_f32(pred_boxes)), _p(num_rois), _stream()), "aug_union")
 
 
 def nms_sorted_dev(boxes, thresh, flags, max_out, keep, num):
