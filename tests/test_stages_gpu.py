@@ -1,6 +1,7 @@
 """Stage-isolated parity of the bandwidth kernels against the oracle (same seeded inputs).
-Integer / index outputs (sort order, NMS survivors, keep lists) must be bit-exact; float outputs are
-checked with the tolerance written at each assert (1e-4 absolute on boxes/scores is the north-star bound)."""
+Integer / index outputs (sort order, NMS survivors, keep lists) and the stages that claim the oracle's fp32 op order
+(box decodes, crop, de-normalised deltas) must be bit-exact; the softmaxes and the spatial mean are held to the
+per-element float64 bounds of stage_ref64.py; other float outputs to the tolerance written at each assert."""
 import os
 
 import numpy as np
@@ -12,6 +13,8 @@ from oracle import boxes as OB
 from oracle import layers as L
 from oracle import nms as ONMS
 from oracle import pipeline as P
+import stage_ref64 as R64
+from stage_ref64 import U as U32, check_guarded, gamma, guarded_out
 
 pytestmark = pytest.mark.gpu
 F = np.float32
@@ -31,27 +34,7 @@ def rand_boxes(rng, n, size=600.0, wh=(8, 200)):
 # SIMT convolutions: each output is one fixed-order chain of K fmaf from 0, then v*scale and + shift rounded once each, so
 # |got - y64| <= |scale| * gamma_K * S + u * (|v*scale| + |v*scale + shift|) per element (classical bound, gamma_K =
 # K u / (1 - K u), S = sum |x||w|; the activation is 1-Lipschitz).  The outputs sit in a NaN-prefilled view between
-# sentinel guard bands.
-U32 = 2.0 ** -24
-GUARD = 64
-SENTINEL = np.int32(0x7fa5a5a5)
-
-
-def gamma(k):
-    return k * U32 / (1 - k * U32)
-
-
-def guarded_out(shape):
-    numel = int(np.prod(shape))
-    buf = torch.full((numel + 2 * GUARD,), int(SENTINEL), dtype=torch.int32, device="cuda")
-    out = buf.view(torch.float32)[GUARD:GUARD + numel].view(shape)
-    out.fill_(float("nan"))
-    return buf, out
-
-
-def check_guarded(buf, numel):
-    b = buf.cpu().numpy()
-    assert (b[:GUARD] == SENTINEL).all() and (b[GUARD + numel:] == SENTINEL).all(), "store outside the output"
+# sentinel guard bands (stage_ref64.guarded_out).
 
 
 def conv64_nhwc(x, w_oihw, stride, pt, pl, ho, wo, groups=1):
@@ -159,7 +142,8 @@ def test_spatial_mean(cuda):
     x = np.random.default_rng(1).standard_normal((33, 7, 7, 256)).astype(F)
     out = torch.empty((33, 256), dtype=torch.float32, device="cuda")
     ops.spatial_mean(dev(x), out)
-    assert np.abs(out.cpu().numpy() - x.mean(axis=(1, 2), dtype=F)).max() < 1e-6
+    m64, bound = R64.spatial_mean_ref(x)
+    print("\n[spatial_mean] max err/bound %.3f" % R64.check_bounded(out.cpu().numpy(), m64, bound, "spatial_mean"))
 
 
 @pytest.mark.parametrize("pre_pool", [0, 1])
@@ -198,8 +182,10 @@ def test_rpn_decode(cuda, scales):
     props = torch.empty((fh * fw * A, 4), dtype=torch.float32, device="cuda")
     base = OA.base_anchors(ratios=(0.5, 1, 2), scales=scales).astype(F)
     ops.rpn_decode(dev(fused), dcol, dev(base), A, fh, fw, 600.0, 800.0, scores, props)
-    assert np.abs(scores.cpu().numpy() - s_want).max() < 1e-6          # 2-way softmax, expf vs np.exp
-    assert np.abs(props.cpu().numpy() - p_want).max() < 1e-4           # north-star box tolerance
+    p64, bound = R64.rpn_fg_ref(cls[0, ..., :A].reshape(-1), cls[0, ..., A:].reshape(-1))
+    r = R64.check_bounded(scores.cpu().numpy(), p64, bound, "fg score")  # 2-way softmax, expf: float64 bound
+    print("\n[rpn_decode A=%d] fg score max err/bound %.3f" % (A, r))
+    R64.check_exact(props.cpu().numpy(), p_want, "proposals")            # the oracle's op order
 
 
 def test_sort_desc_stable(cuda):
@@ -291,7 +277,8 @@ def test_cls_finish_and_bbox_decode(cuda):
     want_prob = L.softmax_lastdim(logits)
     want_bbox = (deltas * np.tile(np.asarray(stds), Cc).astype(F) + np.tile(np.asarray(means), Cc).astype(F)).astype(F)
     assert np.array_equal(cs.cpu().numpy(), logits)
-    assert np.abs(cp.cpu().numpy() - want_prob).max() < 1e-6
+    p64, bound = R64.softmax_ref(logits, R64.cls_depth(Cc))
+    print("\n[cls_finish C=%d] cls_prob max err/bound %.3f" % (Cc, R64.check_bounded(cp.cpu().numpy(), p64, bound, "cls_prob")))
     assert np.array_equal(bp.cpu().numpy(), want_bbox)
     b = rand_boxes(rng, R, 800.0)
     rois = np.hstack([np.zeros((R, 1), F), b]).astype(F)
@@ -299,7 +286,7 @@ def test_cls_finish_and_bbox_decode(cuda):
     _, want_pred = P.im_detect_post(rois, want_prob, want_bbox, scale, 375, 500)
     pred = torch.empty((R, 4 * Cc), dtype=torch.float32, device="cuda")
     ops.bbox_decode(dev(rois), dev(want_bbox), Cc, ops.im_meta_tensor([(scale, 375, 500)]), pred)
-    assert np.abs(pred.cpu().numpy() - want_pred).max() < 1e-4      # north-star box tolerance
+    R64.check_exact(pred.cpu().numpy(), want_pred, "bbox_decode")      # the oracle's op order
 
 
 @pytest.mark.parametrize("R,Cc,gpu_pred", [(300, 21, False), (300, 81, False), (300, 81, True), (1000, 81, False), (17, 5, False)])
