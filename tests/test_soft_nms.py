@@ -223,8 +223,11 @@ def test_abi_rejects_bad_parameters_without_a_device():
     L = _native.lib()
     p = ctypes.c_void_p(64)                     # never dereferenced: the checks come first
 
-    def post(r=300, method=0, sigma=0.5, nt=0.3, thr=0.001):
-        return L.frcnn_detect_post_soft(p, p, p, r, 1, 81, 0.0, method, sigma, nt, thr, 100, 256, p, p, 0, p, p, p, None, 0, None)
+    def post(r=300, method=0, sigma=0.5, nt=0.3, thr=0.001, stride=0):
+        return L.frcnn_detect_post_soft(p, p, p, r, 1, 81, 0.0, method, sigma, nt, thr, 100, 256, p, p, stride, p, p, p, None, 0, None)
+
+    def greedy(r=300, stride=0):
+        return L.frcnn_detect_post(p, p, p, r, 1, 81, 0.0, 0.3, 0, 100, 256, p, p, stride, p, p, p, None, 0, None)
     dets = np.zeros((8193, 5), F)
     out, keep, num = np.zeros((8193, 5), F), np.zeros(8193, np.int32), ctypes.c_int(7)
 
@@ -237,6 +240,9 @@ def test_abi_rejects_bad_parameters_without_a_device():
             assert fn(**bad) == -2, (fn.__name__, bad)
             assert _native.last_error()
     assert post(r=8193) == -5 and "capacity" in _native.last_error()
+    for fn in (post, greedy):                   # both post entries check the record layout and the capacity before any launch
+        assert fn(stride=5) == -2 and "record_stride" in _native.last_error(), fn.__name__
+        assert fn(r=8193) == -5 and "capacity" in _native.last_error(), fn.__name__
     assert host(n=8193) == -5 and "capacity" in _native.last_error()
     assert host(n=0) == 0 and num.value == 0
     assert L.frcnn_soft_nms_host(None, keep.ctypes.data_as(_native.ip), ctypes.byref(num), None, 0, 5, 0, 0.5, 0.3, 0.001, -1) == -2

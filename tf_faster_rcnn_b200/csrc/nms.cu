@@ -764,39 +764,6 @@ extern "C" size_t frcnn_detect_post_workspace_bytes(int r, int num_classes, int 
   return (size_t)batch * num_classes * (size_t)((r + 3) & ~3) * 24 + 256;
 }
 
-extern "C" int frcnn_detect_post(const float* cls_prob, const float* pred_boxes, const int* num_rois, int r, int batch, int num_classes,
-                                 float score_thresh, float nms_thresh, unsigned flags, int max_per_image, int max_det,
-                                 float* det, int* ndet, int record_stride, int* keep, int* keep_cnt, float* keep_score, void* workspace,
-                                 size_t workspace_bytes, void* stream) {
-  FRCNN_REQUIRE(cls_prob && pred_boxes && num_rois && det && ndet && keep && keep_cnt && keep_score, "detect_post: null pointer");
-  FRCNN_REQUIRE(r > 0 && batch > 0 && num_classes >= 2 && num_classes <= 1024, "detect_post: r>0, batch>0, 2<=C<=1024 required");
-  if (r > DET_CAP_BIG) { set_error("detect_post: %d RoIs per image > capacity %d", r, DET_CAP_BIG); return ERR_CAPACITY; }
-  cudaStream_t st = (cudaStream_t)stream;
-  const dim3 grid((unsigned)(num_classes - 1), (unsigned)batch);
-  if (r <= DET_CAP) {
-    class_nms_kernel<DET_CAP, false><<<grid, NMS_THREADS, DET_CAP * 32, st>>>(cls_prob, reinterpret_cast<const float4*>(pred_boxes), num_rois, r,
-                                                                              num_classes, score_thresh, nms_thresh, flags, keep, keep_cnt,
-                                                                              keep_score, nullptr);
-  } else {
-    FRCNN_REQUIRE(workspace && workspace_bytes >= frcnn_detect_post_workspace_bytes(r, num_classes, batch), "detect_post: workspace too small");
-    static bool attr_done = false;
-    if (!attr_done) {
-      FRCNN_CUDA(cudaFuncSetAttribute(class_nms_kernel<DET_CAP_BIG, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, DET_CAP_BIG * 8));
-      attr_done = true;
-    }
-    class_nms_kernel<DET_CAP_BIG, true><<<grid, NMS_THREADS, DET_CAP_BIG * 8, st>>>(
-        cls_prob, reinterpret_cast<const float4*>(pred_boxes), num_rois, r, num_classes, score_thresh, nms_thresh, flags, keep, keep_cnt,
-        keep_score, reinterpret_cast<uint8_t*>(workspace));
-  }
-  FRCNN_LAUNCH_CHECK();
-  FRCNN_REQUIRE(record_stride == 0 || record_stride >= max_det * 6, "detect_post: record_stride %d < max_det*6", record_stride);
-  cap_emit_kernel<<<(unsigned)batch, NMS_THREADS, 0, st>>>(reinterpret_cast<const float4*>(pred_boxes), r, num_classes, max_per_image, max_det,
-                                                          keep, keep_cnt, keep_score, det, ndet,
-                                                          record_stride ? record_stride : max_det * 6, record_stride ? record_stride : 1);
-  FRCNN_LAUNCH_CHECK();
-  return OK;
-}
-
 static int soft_params(int method, float sigma, float nt, float score_thresh, SoftParams* p, const char* who) {
   FRCNN_REQUIRE(method == FRCNN_SOFT_NMS_LINEAR || method == FRCNN_SOFT_NMS_GAUSSIAN || method == FRCNN_SOFT_NMS_HARD,
                 "%s: method %d is not FRCNN_SOFT_NMS_LINEAR / _GAUSSIAN / _HARD", who, method);
@@ -807,17 +774,58 @@ static int soft_params(int method, float sigma, float nt, float score_thresh, So
   return OK;
 }
 
-// the big variant needs more than the default 48 KB of dynamic shared memory; set once per device
+// the big variants need more than the default 48 KB of dynamic shared memory; set once per device
 template <typename K>
-static int soft_smem_attr(K kernel, bool (&done)[MAX_DEVICES]) {
+static int smem_attr_once(K kernel, size_t bytes, bool (&done)[MAX_DEVICES]) {
   int dev = 0;
   FRCNN_CUDA(cudaGetDevice(&dev));
   FRCNN_REQUIRE(dev >= 0 && dev < MAX_DEVICES, "device index %d out of range", dev);
   if (!done[dev]) {
-    FRCNN_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)soft_smem_bytes(DET_CAP_BIG)));
+    FRCNN_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     done[dev] = true;
   }
   return OK;
+}
+
+// Both post entries: the shared checks, then class_stage(grid, st, pred) (its own checks, then the per-class launch), then the cap
+// and the records: image b's count at ndet[b*s], its rows at det + b*s, s = record_stride (0: det [batch, max_det, 6], ndet [batch]).
+template <typename ClassStage>
+static int detect_post_run(const char* who, const float* cls_prob, const float* pred_boxes, const int* num_rois, int r, int batch,
+                           int num_classes, int max_per_image, int max_det, float* det, int* ndet, int record_stride, int* keep,
+                           int* keep_cnt, float* keep_score, void* stream, ClassStage class_stage) {
+  FRCNN_REQUIRE(cls_prob && pred_boxes && num_rois && det && ndet && keep && keep_cnt && keep_score, "%s: null pointer", who);
+  FRCNN_REQUIRE(r > 0 && batch > 0 && num_classes >= 2 && num_classes <= 1024, "%s: r>0, batch>0, 2<=C<=1024 required", who);
+  if (r > DET_CAP_BIG) { set_error("%s: %d RoIs per image > capacity %d", who, r, DET_CAP_BIG); return ERR_CAPACITY; }
+  FRCNN_REQUIRE(record_stride == 0 || record_stride >= max_det * 6, "%s: record_stride %d < max_det*6", who, record_stride);
+  cudaStream_t st = (cudaStream_t)stream;
+  const float4* pred = reinterpret_cast<const float4*>(pred_boxes);
+  if (int rc = class_stage(dim3((unsigned)(num_classes - 1), (unsigned)batch), st, pred)) return rc;
+  FRCNN_LAUNCH_CHECK();
+  cap_emit_kernel<<<(unsigned)batch, NMS_THREADS, 0, st>>>(pred, r, num_classes, max_per_image, max_det, keep, keep_cnt, keep_score, det, ndet,
+                                                          record_stride ? record_stride : max_det * 6, record_stride ? record_stride : 1);
+  FRCNN_LAUNCH_CHECK();
+  return OK;
+}
+
+extern "C" int frcnn_detect_post(const float* cls_prob, const float* pred_boxes, const int* num_rois, int r, int batch, int num_classes,
+                                 float score_thresh, float nms_thresh, unsigned flags, int max_per_image, int max_det,
+                                 float* det, int* ndet, int record_stride, int* keep, int* keep_cnt, float* keep_score, void* workspace,
+                                 size_t workspace_bytes, void* stream) {
+  return detect_post_run("detect_post", cls_prob, pred_boxes, num_rois, r, batch, num_classes, max_per_image, max_det, det, ndet,
+                         record_stride, keep, keep_cnt, keep_score, stream, [&](dim3 grid, cudaStream_t st, const float4* pred) -> int {
+    if (r <= DET_CAP) {
+      class_nms_kernel<DET_CAP, false><<<grid, NMS_THREADS, DET_CAP * 32, st>>>(cls_prob, pred, num_rois, r, num_classes, score_thresh,
+                                                                                nms_thresh, flags, keep, keep_cnt, keep_score, nullptr);
+      return OK;
+    }
+    FRCNN_REQUIRE(workspace && workspace_bytes >= frcnn_detect_post_workspace_bytes(r, num_classes, batch), "detect_post: workspace too small");
+    static bool attr_done[MAX_DEVICES];
+    if (int rc = smem_attr_once(class_nms_kernel<DET_CAP_BIG, true>, DET_CAP_BIG * 8, attr_done)) return rc;
+    class_nms_kernel<DET_CAP_BIG, true><<<grid, NMS_THREADS, DET_CAP_BIG * 8, st>>>(cls_prob, pred, num_rois, r, num_classes, score_thresh,
+                                                                                    nms_thresh, flags, keep, keep_cnt, keep_score,
+                                                                                    reinterpret_cast<uint8_t*>(workspace));
+    return OK;
+  });
 }
 
 extern "C" int frcnn_detect_post_soft(const float* cls_prob, const float* pred_boxes, const int* num_rois, int r, int batch,
@@ -825,31 +833,21 @@ extern "C" int frcnn_detect_post_soft(const float* cls_prob, const float* pred_b
                                       int max_per_image, int max_det, float* det, int* ndet, int record_stride, int* keep,
                                       int* keep_cnt, float* keep_score, void* workspace, size_t workspace_bytes, void* stream) {
   (void)workspace; (void)workspace_bytes;
-  FRCNN_REQUIRE(cls_prob && pred_boxes && num_rois && det && ndet && keep && keep_cnt && keep_score, "detect_post_soft: null pointer");
-  FRCNN_REQUIRE(r > 0 && batch > 0 && num_classes >= 2 && num_classes <= 1024, "detect_post_soft: r>0, batch>0, 2<=C<=1024 required");
-  SoftParams prm;
-  int rc = soft_params(method, sigma, nt, prune_thresh, &prm, "detect_post_soft");
-  if (rc) return rc;
-  FRCNN_REQUIRE(record_stride == 0 || record_stride >= max_det * 6, "detect_post_soft: record_stride %d < max_det*6", record_stride);
-  if (r > DET_CAP_BIG) { set_error("detect_post_soft: %d RoIs per image > capacity %d", r, DET_CAP_BIG); return ERR_CAPACITY; }
-  cudaStream_t st = (cudaStream_t)stream;
-  const dim3 grid((unsigned)(num_classes - 1), (unsigned)batch);
-  const float4* pred = reinterpret_cast<const float4*>(pred_boxes);
-  if (r <= DET_CAP) {
-    class_soft_nms_kernel<SOFT_THREADS, SOFT_PER><<<grid, SOFT_THREADS, soft_smem_bytes(DET_CAP), st>>>(
-        cls_prob, pred, num_rois, r, num_classes, score_thresh, prm, keep, keep_cnt, keep_score);
-  } else {
+  return detect_post_run("detect_post_soft", cls_prob, pred_boxes, num_rois, r, batch, num_classes, max_per_image, max_det, det, ndet,
+                         record_stride, keep, keep_cnt, keep_score, stream, [&](dim3 grid, cudaStream_t st, const float4* pred) -> int {
+    SoftParams prm;
+    if (int rc = soft_params(method, sigma, nt, prune_thresh, &prm, "detect_post_soft")) return rc;
+    if (r <= DET_CAP) {
+      class_soft_nms_kernel<SOFT_THREADS, SOFT_PER><<<grid, SOFT_THREADS, soft_smem_bytes(DET_CAP), st>>>(
+          cls_prob, pred, num_rois, r, num_classes, score_thresh, prm, keep, keep_cnt, keep_score);
+      return OK;
+    }
     static bool attr_done[MAX_DEVICES];
-    rc = soft_smem_attr(class_soft_nms_kernel<SOFT_THREADS_BIG, SOFT_PER_BIG>, attr_done);
-    if (rc) return rc;
+    if (int rc = smem_attr_once(class_soft_nms_kernel<SOFT_THREADS_BIG, SOFT_PER_BIG>, soft_smem_bytes(DET_CAP_BIG), attr_done)) return rc;
     class_soft_nms_kernel<SOFT_THREADS_BIG, SOFT_PER_BIG><<<grid, SOFT_THREADS_BIG, soft_smem_bytes(DET_CAP_BIG), st>>>(
         cls_prob, pred, num_rois, r, num_classes, score_thresh, prm, keep, keep_cnt, keep_score);
-  }
-  FRCNN_LAUNCH_CHECK();
-  cap_emit_kernel<<<(unsigned)batch, NMS_THREADS, 0, st>>>(pred, r, num_classes, max_per_image, max_det, keep, keep_cnt, keep_score, det,
-                                                          ndet, record_stride ? record_stride : max_det * 6, record_stride ? record_stride : 1);
-  FRCNN_LAUNCH_CHECK();
-  return OK;
+    return OK;
+  });
 }
 
 extern "C" int frcnn_soft_nms_host(float* dets_out, int* keep_out, int* num_out, const float* dets_host, int n, int dim, int method,
@@ -867,7 +865,7 @@ extern "C" int frcnn_soft_nms_host(float* dets_out, int* keep_out, int* num_out,
   const int dev = device_id < 0 ? cur : device_id;
   if (cur != dev) FRCNN_CUDA(cudaSetDevice(dev));
   static bool attr_done[MAX_DEVICES];
-  if (n > DET_CAP) rc = soft_smem_attr(soft_nms_set_kernel<SOFT_THREADS_BIG, SOFT_PER_BIG>, attr_done);
+  if (n > DET_CAP) rc = smem_attr_once(soft_nms_set_kernel<SOFT_THREADS_BIG, SOFT_PER_BIG>, soft_smem_bytes(DET_CAP_BIG), attr_done);
   float* din = nullptr; float* dout = nullptr; int* dkeep = nullptr;
   cudaError_t e = cudaSuccess;
   if (!rc) {

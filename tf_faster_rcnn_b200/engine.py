@@ -9,6 +9,7 @@ Layer semantics follow lib/nets/network.py:233-262 (graph order), :323-378 (head
 backbones emit their layers through the Tape from lib/nets/{vgg16,resnet_v1,mobilenet_v1}.py's
 counterparts in tf_faster_rcnn_b200/lib/nets/.
 """
+import collections
 import ctypes
 import os
 
@@ -198,8 +199,104 @@ class Tape:
 
 REC_HEADER = 8     # 4-byte words in front of every image's detection rows: word 0 = int32 detection count
 
+# the options the post step is built for; a change rebuilds it (PostStage._ensure_post).  soft_nms: soft_nms_args() or None
+PostKey = collections.namedtuple("PostKey", "score_thresh nms_thresh use_gpu_nms max_per_image soft_nms")
 
-class ShapePlan:
+
+class PostStage:
+    """The test_net tail of a plan whose im_detect outputs are `cls_prob`, `pred_boxes` and `num_rois` (`batch` images of `R`
+    rows): the per-class NMS or Soft-NMS into `keep` / `keep_cnt` / `keep_score` (`post_ws`: the greedy NMS's workspace), the
+    max_per_image cap and the detection records, built on first use for the options in force; in feature mode also the
+    per-detection gather of `fc7`.  The subclass allocates those buffers.  Two record buffers: with `double_buffer`,
+    consecutive detect launches alternate between them.  Also the plan's CUDA-graph cache."""
+
+    def __init__(self, net, batch, use_graph):
+        self.net, self.batch = net, batch
+        self.post_key = None
+        self.recs = [None, None]
+        self.rec = self.ndet = None    # views of the buffer the LAST detect launch wrote
+        self.post_steps = [None, None]
+        self.feat_out = self.roi_out = self.features_step = None   # feature mode (_ensure_post(features=True))
+        self.double_buffer = False
+        self.slot = 0
+        self.max_det = 0
+        self.graphs = {}
+        self.use_graph = use_graph
+
+    def _ensure_post(self, features=False):
+        """(Re)build the detection-record buffers and the post step for the current score / NMS thresholds, cap and Soft-NMS
+        setting; with `features`, also the per-detection feature buffers and their gather step."""
+        o = self.net.options
+        soft = o.get("soft_nms")
+        key = PostKey(float(o["score_thresh"]), float(o["nms_thresh"]), bool(o["use_gpu_nms"]), int(o["max_per_image"]),
+                      None if soft is None else soft_nms_args(*soft))
+        if key != self.post_key:
+            self._build_post(key)
+        if features and self.features_step is None:
+            check_feature_mode(key.max_per_image)
+            C, B, fdim = self.net.num_classes, self.batch, int(self.fc7.shape[1])
+            # feat_out [B, max_det, F]: row k of image b = fc7 row of record row k; roi_out [B, max_det] int32 (-1 past the count)
+            self.feat_out = ops.zeros((B, self.max_det, fdim))
+            self.roi_out = ops.zeros((B, self.max_det), dtype=torch.int32)
+            self.features_step = lambda: ops.detect_features(self.keep, self.keep_cnt, self.fc7, C, self.feat_out, self.roi_out)
+
+    def _build_post(self, key):
+        C, R, B = self.net.num_classes, self.R, self.batch
+        mpi, soft = key.max_per_image, key.soft_nms
+        # records: max_per_image survivors + head-room for ties at the threshold score; no cap -> every (roi, class) pair.
+        # A record set that still does not fit is reported through ndet > max_det and raised on the host (never truncated).
+        self.max_det = max_det = 2 * mpi + 56 if mpi > 0 else R * (C - 1)
+        thr, flags = nms_threshold(key.nms_thresh, key.use_gpu_nms)
+
+        def make_post(rec):
+            # as_strided: view() repacks a size-1 batch dimension, which would drop the record stride at batch 1
+            det, ndet = rec.as_strided((B, max_det, 6), (rec.stride(0), 6, 1), REC_HEADER), rec.view(torch.int32)[:, 0]
+            if soft is not None:
+                return lambda: ops.detect_post_soft(self.cls_prob, self.pred_boxes, self.num_rois, C, key.score_thresh, soft[0], soft[1],
+                                                    float(F(key.nms_thresh)), soft[2], mpi, det, ndet, self.keep, self.keep_cnt,
+                                                    self.keep_score, batch=B)
+            return lambda: ops.detect_post(self.cls_prob, self.pred_boxes, self.num_rois, C, key.score_thresh, thr, flags, mpi, det, ndet,
+                                           self.keep, self.keep_cnt, self.keep_score, self.post_ws, batch=B)
+        self.recs = [ops.zeros((B, REC_HEADER + max_det * 6)) for _ in range(2)]
+        self.post_steps = [make_post(r) for r in self.recs]
+        self.post_key = key
+        self._select(0)
+        self.graphs.pop(("detect", 0), None); self.graphs.pop(("detect", 1), None)
+        self.feat_out = self.roi_out = self.features_step = None
+        self.graphs.pop(("features", 0), None)
+
+    def _select(self, slot):
+        self.slot = slot
+        self.rec = self.recs[slot]
+        self.ndet = self.rec.view(torch.int32)[:, 0]
+
+    def _begin_post(self, features=False):
+        """Build the post step if the options changed and pick this launch's record buffer: the other one with `double_buffer`,
+        else buffer 0 (always 0 in feature mode, which does not double-buffer)."""
+        self._ensure_post(features)
+        self._select(self.slot ^ 1 if self.double_buffer and not features else 0)
+
+    def _replay(self, gkey, fns):
+        """Run the launch list fns: as the CUDA graph cached under gkey (captured on first use, after one eager warm-up pass
+        for function attributes and lazy allocations), or eagerly without graphs."""
+        if not self.use_graph:
+            for fn in fns:
+                fn()
+            return
+        g = self.graphs.get(gkey)
+        if g is None:
+            for fn in fns:
+                fn()
+            torch.cuda.current_stream().synchronize()
+            g = self.graphs[gkey] = LaunchGraph(fns)
+        g.replay()
+
+    def records(self):
+        """Host copy of the detection records of the batch after a 'detect' launch: list of [n,6] arrays (one D2H copy)."""
+        return split_host_records(self.rec.cpu(), self.max_det)
+
+
+class ShapePlan(PostStage):
     """Everything needed to run `batch` images of one blob shape: static input/output buffers, the tape, its CUDA graphs.
 
     The reference graph is batch 1 (lib/nets/network.py:388); batch > 1 is the throughput mode (SURVEY 8(f) rank 4): the
@@ -212,7 +309,8 @@ class ShapePlan:
     set_boxes() instead of the RPN's proposals; the RPN is not built and the head / im_detect tail are the same steps."""
 
     def __init__(self, net, h, w, batch=1, use_graph=True, rois_source="rpn", cap=None):
-        self.net, self.h, self.w, self.batch = net, h, w, batch
+        super().__init__(net, batch, use_graph)
+        self.h, self.w = h, w
         cfgd = net.options
         wts = net.weights
         t = Tape(wts)
@@ -270,16 +368,6 @@ class ShapePlan:
         self.keep = t.new(B, C, R, dtype=torch.int32); self.keep_cnt = t.new(B, C, dtype=torch.int32)
         self.keep_score = t.new(B, C, R)
         self.post_ws = ops.detect_post_workspace(R, C, B); t.bufs.append(self.post_ws)
-        self.post_key = None
-        self.recs = [None, None]       # two record buffers; `double_buffer` makes consecutive detect launches alternate
-        self.rec = self.det = self.ndet = None   # ... views of the buffer the LAST detect launch wrote
-        self.post_steps = [None, None]
-        self.feat_out = self.roi_out = self.features_step = None   # feature mode (_ensure_post(features=True))
-        self.double_buffer = False
-        self.slot = 0
-        self.max_det = 0
-        self.graphs = {}
-        self.use_graph = use_graph
 
     def _caller_rois(self, t, cap):
         """RoIs from caller boxes: [batch, cap, 4] boxes + int32 counts staged through a pinned ring (set_boxes)."""
@@ -359,73 +447,16 @@ class ShapePlan:
         self.tape.bufs = []
         self.post_steps = [None, None]
         self.recs = [None, None]
-        self.rec = self.det = self.ndet = None
+        self.rec = self.ndet = None
         self.feat_out = self.roi_out = self.features_step = None
-
-    def _ensure_post(self, features=False):
-        """(Re)build the detection-record buffers and the post step for the current score / NMS thresholds, cap and Soft-NMS
-        setting; with `features`, also the per-detection feature buffers and their gather step."""
-        o = self.net.options
-        soft = o.get("soft_nms")
-        key = (float(o["score_thresh"]), float(o["nms_thresh"]), bool(o["use_gpu_nms"]), int(o["max_per_image"]),
-               None if soft is None else soft_nms_args(*soft))
-        if key != self.post_key:
-            self._build_post(key)
-        if features and self.features_step is None:
-            check_feature_mode(key[3])
-            C, B, fdim = self.net.num_classes, self.batch, int(self.fc7.shape[1])
-            # feat_out [B, max_det, F]: row k of image b = fc7 row of record row k; roi_out [B, max_det] int32 (-1 past the count)
-            self.feat_out = ops.zeros((B, self.max_det, fdim))
-            self.roi_out = ops.zeros((B, self.max_det), dtype=torch.int32)
-            self.features_step = lambda: ops.detect_features(self.keep, self.keep_cnt, self.fc7, C, self.feat_out, self.roi_out)
-
-    def _build_post(self, key):
-        net = self.net
-        C, R, B = net.num_classes, self.R, self.batch
-        mpi = key[3]
-        # records: max_per_image survivors + head-room for ties at the threshold score; no cap -> every (roi, class) pair.
-        # A record set that still does not fit is reported through ndet > max_det and raised on the host (never truncated).
-        self.max_det = 2 * mpi + 56 if mpi > 0 else R * (C - 1)
-        stride = REC_HEADER + self.max_det * 6
-        thr, flags = nms_threshold(key[1], key[2])
-        soft = key[4]
-
-        def make_post(rec):
-            def post():
-                if soft is not None:
-                    N.check(N.lib().frcnn_detect_post_soft(ops._p(self.cls_prob), ops._p(self.pred_boxes), ops._p(self.num_rois), R, B, C,
-                                                           key[0], soft[0], soft[1], float(F(key[1])), soft[2], mpi, self.max_det,
-                                                           C_void(rec.data_ptr() + 4 * REC_HEADER), ops._p(rec), stride,
-                                                           ops._p(self.keep), ops._p(self.keep_cnt), ops._p(self.keep_score), None, 0,
-                                                           ops._stream()), "detect_post_soft")
-                    return
-                N.check(N.lib().frcnn_detect_post(ops._p(self.cls_prob), ops._p(self.pred_boxes), ops._p(self.num_rois), R, B, C, key[0],
-                                                  thr, flags, mpi, self.max_det, C_void(rec.data_ptr() + 4 * REC_HEADER), ops._p(rec), stride,
-                                                  ops._p(self.keep), ops._p(self.keep_cnt), ops._p(self.keep_score), ops._p(self.post_ws),
-                                                  self.post_ws.numel(), ops._stream()), "detect_post")
-            return post
-        self.recs = [ops.zeros((B, stride)) for _ in range(2)]
-        self.post_steps = [make_post(r) for r in self.recs]
-        self.post_key = key
-        self._select(0)
-        self.graphs.pop(("detect", 0), None); self.graphs.pop(("detect", 1), None)
-        self.feat_out = self.roi_out = self.features_step = None
-        self.graphs.pop(("features", 0), None)
-
-    def _select(self, slot):
-        self.slot = slot
-        self.rec = self.recs[slot]
-        self.det = [self.rec[b, REC_HEADER:].view(self.max_det, 6) for b in range(self.batch)]
-        self.ndet = self.rec.view(torch.int32)[:, 0]
 
     def steps_for(self, mode):
         """mode: 'test_image' (network outputs), 'im_detect' (+ decoded boxes), 'detect' (+ per-class NMS, cap, records),
-        'features' (+ the head feature and RoI index of every record row)."""
+        'features' (+ the head feature and RoI index of every record row); the last two after _begin_post."""
         if mode == "test_image":
             return [fn for _, fn in self.tape.steps[:self.n_test_image_steps]]
         fns = [fn for _, fn in self.tape.steps[:self.n_im_detect_steps]]
         if mode in ("detect", "features"):
-            self._ensure_post(features=mode == "features")
             fns.append(self.post_steps[self.slot])
         if mode == "features":
             fns.append(self.features_step)
@@ -450,52 +481,29 @@ class ShapePlan:
             self.set_meta(meta)
         gkey = mode
         if mode in ("detect", "features"):
-            self._ensure_post(features=features)
-            self._select(self.slot ^ 1 if self.double_buffer and not features else 0)
+            self._begin_post(features)
             gkey = (mode, self.slot)
-        if self.use_graph:
-            g = self.graphs.get(gkey)
-            if g is None:
-                fns = self.steps_for(mode)
-                for fn in fns:                        # warm-up: function attributes, lazy allocations
-                    fn()
-                torch.cuda.current_stream().synchronize()
-                g = LaunchGraph(fns)
-                self.graphs[gkey] = g
-            g.replay()
-        else:
-            for fn in self.steps_for(mode):
-                fn()
-
-    def records(self):
-        """Host copy of the detection records of the batch after a 'detect' launch: list of [n,6] arrays (one D2H copy)."""
-        return split_host_records(self.rec.cpu(), self.max_det)
+        self._replay(gkey, self.steps_for(mode))
 
 
-AUG_MAX_ROIS = 8192    # RoI rows per image that frcnn_detect_post / _soft take: the cap of the union
+AUG_MAX_ROIS = 8192    # RoI rows per image that the post step (ops.detect_post / _soft) takes: the cap of the union
 
 
-class AugPlan:
+class AugPlan(PostStage):
     """Test-time augmentation (TEST.BBOX_AUG) for `batch` images whose views have the blob shapes `views` = ((h, w, flip), ...),
     in union order.  Views of one blob shape share one ShapePlan at batch k*batch from the network's plan cache: unflipped views
     take the first slots, so an identity view and its flip are slots [0, B) and [B, 2B) of a batch-2B plan.  One call replays
     the sub-plans' im_detect graphs, then frcnn_aug_union merges the views' rows into the union buffers and the post step runs
-    on them.  The union, the post step and its two alternating record buffers are this object's; the post step is ShapePlan's
-    own construction (the methods below are ShapePlan's), run on R = the sum of the views' rows."""
-
-    _ensure_post = ShapePlan._ensure_post
-    _build_post = ShapePlan._build_post
-    _select = ShapePlan._select
-    records = ShapePlan.records
+    on them.  The union, the post step and its two alternating record buffers are this object's; the post step is the same
+    PostStage as a ShapePlan's, run on R = the sum of the views' rows."""
 
     def __init__(self, net, views, batch):
-        self.net, self.views, self.batch = net, tuple(views), int(batch)
+        super().__init__(net, int(batch), net.use_cuda_graph)
+        self.views = tuple(views)
         B, C = self.batch, net.num_classes
         self.shapes, self.view_slot, counts = aug_groups(self.views)
         self.group_batch = {hw: k * B for hw, k in counts.items()}
         self.subs = {}
-        self.graphs = {}
-        self.use_graph = net.use_cuda_graph
         self.bind()
         self.rows = [self.subs[(h, w)].R for h, w, _ in self.views]
         R = self.R = sum(self.rows)
@@ -504,14 +512,6 @@ class AugPlan:
         self.keep = ops.zeros((B, C, R), dtype=torch.int32); self.keep_cnt = ops.zeros((B, C), dtype=torch.int32)
         self.keep_score = ops.zeros((B, C, R))
         self.post_ws = ops.detect_post_workspace(R, C, B)
-        self.post_key = None
-        self.recs = [None, None]
-        self.rec = self.det = self.ndet = None
-        self.post_steps = [None, None]
-        self.feat_out = self.roi_out = self.features_step = None
-        self.double_buffer = False
-        self.slot = 0
-        self.max_det = 0
 
     def bind(self):
         """Fetch the sub-plans from the network's plan cache (marking them recently used).  A plan evicted by the LRU and rebuilt
@@ -556,20 +556,8 @@ class AugPlan:
         if not detect:
             self._union()
             return
-        self._ensure_post()
-        self._select(self.slot ^ 1 if self.double_buffer else 0)
-        fns = [self._union, self.post_steps[self.slot]]
-        if not self.use_graph:
-            for fn in fns:
-                fn()
-            return
-        g = self.graphs.get(("detect", self.slot))
-        if g is None:
-            for fn in fns:
-                fn()
-            torch.cuda.current_stream().synchronize()
-            g = self.graphs[("detect", self.slot)] = LaunchGraph(fns)
-        g.replay()
+        self._begin_post()
+        self._replay(("detect", self.slot), [self._union, self.post_steps[self.slot]])
 
 
 def aug_groups(views):

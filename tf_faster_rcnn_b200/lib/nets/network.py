@@ -178,6 +178,13 @@ class Network(object):
         aug.launch(im_scales, orig_hws, detect=True)
         return aug.records(), aug
 
+    def _batch_plan(self, images, im_scales, orig_hws, cap=None):
+        """A batch call's arguments checked (images [B, H, W, 3], B scale factors, B original (h, w)) -> (plan_for that shape,
+        batch and cap; the B per-image (scale, orig_h, orig_w) meta rows)."""
+        assert images.shape[3] == 3 and len(im_scales) == len(orig_hws) == images.shape[0]
+        meta = [(float(s), int(hw[0]), int(hw[1])) for s, hw in zip(im_scales, orig_hws)]
+        return self.plan_for(images.shape[1], images.shape[2], len(meta), cap=cap), meta
+
     def _copy_in(self, plan, image):
         if isinstance(image, torch.Tensor):
             plan.image.copy_(image, non_blocking=True)
@@ -201,11 +208,9 @@ class Network(object):
     def detect_batch(self, images, im_scales, orig_hws):
         """Throughput path: `images` [B,H,W,3] blobs of ONE shape (numpy or a pinned torch tensor), per-image scale factors and
         original (h, w).  -> (list of B det arrays [n,6], plan).  The reference is batch 1; this is SURVEY 8(f) rank 4."""
-        b = int(images.shape[0])
-        assert images.shape[3] == 3 and len(im_scales) == b and len(orig_hws) == b
-        plan = self.plan_for(images.shape[1], images.shape[2], b)
+        plan, meta = self._batch_plan(images, im_scales, orig_hws)
         self._copy_in(plan, images)
-        plan.launch(post=True, detect=True, meta=[(float(im_scales[i]), int(orig_hws[i][0]), int(orig_hws[i][1])) for i in range(b)])
+        plan.launch(post=True, detect=True, meta=meta)
         return plan.records(), plan
 
     # ---- region features: per-detection head features, and scoring of caller-supplied boxes ---------------------------------
@@ -214,27 +219,23 @@ class Network(object):
         MobileNet) and the index of the RoI it came from, gathered on the device in the same graph replay.
         -> (list over images of (det [n,6], feats [n,F] fp32, roi_index [n] int32), plan); det equals detect_batch's records.
         Needs options['max_per_image'] > 0."""
-        b = int(images.shape[0])
-        assert images.shape[3] == 3 and len(im_scales) == b and len(orig_hws) == b
         _no_bbox_aug("per-detection features (detect_features)")
         engine.check_feature_mode(int(self.options["max_per_image"]))
-        plan = self.plan_for(images.shape[1], images.shape[2], b)
+        plan, meta = self._batch_plan(images, im_scales, orig_hws)
         self._copy_in(plan, images)
-        plan.launch(post=True, features=True, meta=[(float(im_scales[i]), int(orig_hws[i][0]), int(orig_hws[i][1])) for i in range(b)])
+        plan.launch(post=True, features=True, meta=meta)
         dets = plan.records()
         feats, rois = plan.feat_out.cpu(), plan.roi_out.cpu()
         return [(d, feats[i, :d.shape[0]].numpy().copy(), rois[i, :d.shape[0]].numpy().copy()) for i, d in enumerate(dets)], plan
 
     def _run_boxes(self, images, im_scales, orig_hws, boxes):
         """Enqueue `images` [B,H,W,3] with caller boxes as the RoIs on a caller-box plan (no sync) -> plan."""
-        b = int(images.shape[0])
-        assert images.shape[3] == 3 and len(im_scales) == b and len(orig_hws) == b
         _no_bbox_aug("caller boxes (score_boxes / im_detect(boxes=))")
-        boxes = engine.check_boxes(boxes, b)
-        plan = self.plan_for(images.shape[1], images.shape[2], b, cap=engine.box_capacity(max(a.shape[0] for a in boxes)))
+        boxes = engine.check_boxes(boxes, int(images.shape[0]))
+        plan, meta = self._batch_plan(images, im_scales, orig_hws, cap=engine.box_capacity(max(a.shape[0] for a in boxes)))
         self._copy_in(plan, images)
         plan.set_boxes(boxes)
-        plan.launch(post=True, meta=[(float(im_scales[i]), int(orig_hws[i][0]), int(orig_hws[i][1])) for i in range(b)])
+        plan.launch(post=True, meta=meta)
         return plan
 
     def score_boxes(self, images, im_scales, orig_hws, boxes):
@@ -255,9 +256,7 @@ class Network(object):
         and copies the records into one of two pinned host buffers.  -> ticket for collect_batch().  At most TWO tickets may be
         outstanding (submit i+1, collect i, submit i+2, ...): that is what keeps the copy of batch i+1 under the compute of
         batch i.  Results are identical to detect_batch()."""
-        b = int(images.shape[0])
-        assert images.shape[3] == 3 and len(im_scales) == b and len(orig_hws) == b
-        plan = self.plan_for(images.shape[1], images.shape[2], b)
+        plan, meta = self._batch_plan(images, im_scales, orig_hws)
         pipe = plan.__dict__.setdefault("_pipe", None)
         if pipe is None:
             pipe = plan._pipe = dict(copy_stream=torch.cuda.Stream(), stage=[torch.empty_like(plan.image) for _ in range(2)],
@@ -276,7 +275,7 @@ class Network(object):
         plan.image.copy_(pipe["stage"][k], non_blocking=True)             # device-to-device: ~microseconds, keeps the graph's input address fixed
         pipe["consumed"][k].record(main)
         pipe["used"][k] = True
-        plan.launch(post=True, detect=True, meta=[(float(im_scales[i]), int(orig_hws[i][0]), int(orig_hws[i][1])) for i in range(b)])
+        plan.launch(post=True, detect=True, meta=meta)
         if pipe["host"][k] is None or pipe["host"][k].shape != plan.rec.shape:
             pipe["host"][k] = torch.empty(plan.rec.shape, dtype=torch.float32).pin_memory()
         pipe["host"][k].copy_(plan.rec, non_blocking=True)

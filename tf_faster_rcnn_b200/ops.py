@@ -220,15 +220,24 @@ def detect_post_workspace(r, num_classes, batch=1):
     return torch.empty(int(N.lib().frcnn_detect_post_workspace_bytes(r, num_classes, batch)), dtype=torch.uint8, device="cuda")
 
 
+def _record_stride(det, ndet):
+    """record_stride of the post entries: 0 for a packed det [batch, max_det, 6] beside its own ndet; for det rows inside
+    record buffers (image b's record = int32 count ndet[b], then its rows det[b]) the distance between two records, in floats."""
+    if det.dim() == 2 or det.stride(0) == det.shape[1] * 6:
+        return 0
+    assert det.stride()[1:] == (6, 1) and ndet.stride(0) == det.stride(0), "det / ndet are not views of one record buffer"
+    return det.stride(0)
+
+
 def detect_post(cls_prob, pred_boxes, num_rois, num_classes, score_thresh, nms_thresh, flags, max_per_image, det, ndet, keep,
                 keep_cnt, keep_score, workspace=None, batch=1):
     """cls_prob [batch*r, C]; det [batch, max_det, 6] (or [max_det, 6] for batch 1); ndet int32 [batch] = TRUE counts
-    (a count above max_det means the records did not fit)."""
+    (a count above max_det means the records did not fit).  det and ndet may be views of record buffers (_record_stride)."""
     r = cls_prob.shape[0] // batch
     max_det = det.shape[-2]
     N.check(N.lib().frcnn_detect_post(_p(cls_prob), _p(pred_boxes), _p(num_rois), r, batch, num_classes, float(score_thresh),
-                                      float(nms_thresh), flags, max_per_image, max_det, _p(det), _p(ndet), 0, _p(keep),
-                                      _p(keep_cnt), _p(keep_score), _p(workspace), 0 if workspace is None else workspace.numel(),
+                                      float(nms_thresh), flags, max_per_image, max_det, _p(det), _p(ndet), _record_stride(det, ndet),
+                                      _p(keep), _p(keep_cnt), _p(keep_score), _p(workspace), 0 if workspace is None else workspace.numel(),
                                       _stream()), "detect_post")
 
 
@@ -239,7 +248,8 @@ def detect_post_soft(cls_prob, pred_boxes, num_rois, num_classes, score_thresh, 
     max_det = det.shape[-2]
     N.check(N.lib().frcnn_detect_post_soft(_p(cls_prob), _p(pred_boxes), _p(num_rois), r, batch, num_classes, float(score_thresh),
                                            int(method), float(sigma), float(nt), float(prune_thresh), max_per_image, max_det, _p(det),
-                                           _p(ndet), 0, _p(keep), _p(keep_cnt), _p(keep_score), None, 0, _stream()), "detect_post_soft")
+                                           _p(ndet), _record_stride(det, ndet), _p(keep), _p(keep_cnt), _p(keep_score), None, 0,
+                                           _stream()), "detect_post_soft")
 
 
 def detect_features(keep, keep_cnt, fc7, num_classes, feat_out, roi_out):
