@@ -13,8 +13,9 @@ from oracle import boxes as OB
 from oracle import layers as L
 from oracle import nms as ONMS
 from oracle import pipeline as P
+import front_ref64 as F64
 import stage_ref64 as R64
-from stage_ref64 import U as U32, check_guarded, gamma, guarded_out
+from stage_ref64 import check_guarded, guarded_out
 
 pytestmark = pytest.mark.gpu
 F = np.float32
@@ -37,24 +38,8 @@ def rand_boxes(rng, n, size=600.0, wh=(8, 200)):
 # sentinel guard bands (stage_ref64.guarded_out).
 
 
-def conv64_nhwc(x, w_oihw, stride, pt, pl, ho, wo, groups=1):
-    xt = torch.from_numpy(x.astype(np.float64)).permute(0, 3, 1, 2)
-    kh, kw = w_oihw.shape[2:]
-    pb = max((ho - 1) * stride + kh - x.shape[1] - pt, 0)
-    pr = max((wo - 1) * stride + kw - x.shape[2] - pl, 0)
-    xt = torch.nn.functional.pad(xt, (pl, pr, pt, pb))
-    y = torch.nn.functional.conv2d(xt, torch.from_numpy(w_oihw.astype(np.float64)), None, stride=stride, groups=groups)
-    return y.permute(0, 2, 3, 1).numpy()[:, :ho, :wo]
-
-
 def check_fma_chain(got, x, w_oihw, stride, pt, pl, ho, wo, K, scale, shift, act, groups=1):
-    v = conv64_nhwc(x, w_oihw, stride, pt, pl, ho, wo, groups)
-    S = conv64_nhwc(np.abs(x), np.abs(w_oihw), stride, pt, pl, ho, wo, groups)
-    sc = np.ones(v.shape[-1]) if scale is None else scale.astype(np.float64)
-    a = v * sc
-    b = a + shift.astype(np.float64)
-    y = np.maximum(b, 0) if act == 1 else np.minimum(np.maximum(b, 0), 6)
-    bound = (np.abs(sc) * gamma(K) * S + U32 * (np.abs(a) + np.abs(b))) * (1 + 4 * K * U32) + 1e-37
+    y, bound = F64.fma_chain_ref(x, w_oihw, stride, pt, pl, ho, wo, K, scale, shift, act, groups)
     err = np.abs(got.astype(np.float64) - y)
     assert np.isfinite(got).all(), "unwritten output"
     assert (err <= bound).all(), "max err/bound %.3g" % (err / bound).max()
