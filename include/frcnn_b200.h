@@ -257,6 +257,62 @@ int frcnn_detect_post_soft(const float* cls_prob_dev, const float* pred_boxes_de
                            int num_classes, float score_thresh, int method, float sigma, float nt, float prune_thresh,
                            int max_per_image, int max_det, float* det_dev, int* ndet_dev, int record_stride, int* keep_dev,
                            int* keep_cnt_dev, float* keep_score_dev, void* workspace_dev, size_t workspace_bytes, void* stream);
+/* Box voting (Detectron's TEST.BBOX_VOTE, box_voting) between the per-class NMS / Soft-NMS and the max_per_image cap: each kept
+ * box is replaced by the score-weighted average of the candidates of its class that overlap it, and optionally so is its score.
+ * An extension beyond the reference.  For one set, the top boxes t (the NMS / Soft-NMS output, with its scores) and the candidates
+ * a[0..n) (the rows NMS started from, with their ORIGINAL scores s_a), every fp32 step a separate round-to-nearest operation:
+ *   ov(t, a): iw = (min(t.x2,a.x2) - max(t.x1,a.x1)) + 1; if iw > 0: ih = (min(t.y2,a.y2) - max(t.y1,a.y1)) + 1; if ih > 0:
+ *             ov = (iw*ih) / ((area(t) + area(a)) - iw*ih), area(u) = ((u.x2-u.x1)+1) * ((u.y2-u.y1)+1)  (Soft-NMS's overlap);
+ *             otherwise ov = 0.
+ *   V(t) = { a : ov(t, a) >= thresh }, n = |V(t)|, thresh in (0, 1].
+ *   Sums over V(t) in fp64 (each fp32 product below is exact in fp64), in this order: candidate k goes to partial k mod 32, each
+ *   partial adds its candidates in ascending k starting from +0, then the 32 partials P are combined by the butterfly
+ *   P[l] = P[l] + P[l ^ o] for o = 16, 8, 4, 2, 1 (every l at once), and the result is P[0]:
+ *     S = sum s_a;  X1 = sum s_a*a.x1 (and Y1, X2, Y2);
+ *     IOU_AVG: M0 = sum ov*s_a, M1 = sum ov;  GENERALIZED_AVG: M0 = sum exp(beta*s_a);
+ *     TEMP_AVG: M0 = sum e0/(e0+e1), q = 1-s_a, m = max(s_a, q), e0 = exp(log(s_a/m)/beta), e1 = exp(log(q/m)/beta).
+ *   Box: (X1/S, Y1/S, X2/S, Y2/S), each an fp64 division rounded once to fp32.
+ *   Score, computed in fp64 and rounded once to fp32:  ID: unchanged (the NMS / Soft-NMS score);  AVG: S/n;  IOU_AVG: M0/M1;
+ *     GENERALIZED_AVG: log(M0/n)/beta;  QUASI_SUM: S/n^beta;  TEMP_AVG: M0/n  (beta finite and > 0).  n^beta is n for beta 1,
+ *     n*n for beta 2 and sqrt(n) for beta 0.5 (all exact or correctly rounded), else pow(n, beta).  exp, log and pow are the fp64
+ *     library functions, within an ulp or two of the exact value, so an output may differ from another libm's in its last bit.
+ *   Choices of this implementation: n = 0 (possible through frcnn_box_vote_host only: on the post path every top box is a
+ *   candidate and overlaps itself with ov = 1) keeps the box and the score, where Detectron divides by zero; S = 0 (zero scores)
+ *   keeps the box.  Detectron accumulates in float32; these fp64 sums are at least as accurate.
+ * In the post entries the candidates are the stage's own (score > score_thresh, ascending RoI order) and the top boxes the kept
+ * list keep / keep_score [0, keep_cnt) of each class.  For every method except ID each class list is then re-sorted stably by
+ * descending voted score (ties keep the NMS order), so that it is again sorted by descending score, which the cap needs: the cap
+ * counts scores >= t by binary search and finds the max_per_image-th score by a bitwise search on the fp32 pattern, valid when
+ * every score is >= +0.  Voted scores are: AVG, QUASI_SUM > 0 (positive scores); IOU_AVG > 0 (ov >= thresh > 0); GENERALIZED_AVG
+ * = log(mean(exp(beta*s)))/beta >= log(1)/beta = +0; TEMP_AVG a mean of e0/(e0+e1) in [+0, 1] -- never -0 and never NaN for
+ * scores in [0, 1] and beta > 0.  The record set after the cap equals Detectron's (vote, then cap); only the row order within a
+ * class is the voted-score order instead of Detectron's NMS order. */
+#define FRCNN_BOX_VOTE_ID 0
+#define FRCNN_BOX_VOTE_AVG 1
+#define FRCNN_BOX_VOTE_IOU_AVG 2
+#define FRCNN_BOX_VOTE_GENERALIZED_AVG 3
+#define FRCNN_BOX_VOTE_QUASI_SUM 4
+#define FRCNN_BOX_VOTE_TEMP_AVG 5
+/* host buffers, synchronous, one set: top_host [n_top, top_dim >= 5] and all_host [n_all, all_dim >= 5] rows (x1, y1, x2, y2,
+ * score, ...).  dets_out [n_top, 5] = the voted rows in top_host's row order (no re-sort).  n_all <= 8192 (else
+ * FRCNN_ERR_CAPACITY).  An unknown method, thresh outside (0, 1] or beta not finite and > 0 give FRCNN_ERR_ARG.  device_id < 0:
+ * the calling thread's current device; the caller's current device is left unchanged. */
+int frcnn_box_vote_host(float* dets_out, const float* top_host, int n_top, int top_dim, const float* all_host, int n_all,
+                        int all_dim, float thresh, int method, float beta, int device_id);
+/* frcnn_detect_post / frcnn_detect_post_soft with box voting between the per-class stage and the cap.  vote_box_dev [batch, C, r]
+ * float4 (16-byte aligned): entry (b, c, j) = the voted box of keep_dev[b, c, j] for j < the class's count before the cap; the
+ * records take their boxes from it.  keep_score_dev holds the voted scores and keep_dev the re-sorted order (methods other than
+ * ID), so frcnn_detect_features stays consistent with the record rows. */
+int frcnn_detect_post_vote(const float* cls_prob_dev, const float* pred_boxes_dev, const int* num_rois_dev, int r, int batch,
+                           int num_classes, float score_thresh, float nms_thresh, unsigned flags, int max_per_image, int max_det,
+                           float* det_dev, int* ndet_dev, int record_stride, int* keep_dev, int* keep_cnt_dev, float* keep_score_dev,
+                           void* workspace_dev, size_t workspace_bytes, float vote_thresh, int vote_method, float vote_beta,
+                           float* vote_box_dev, void* stream);
+int frcnn_detect_post_soft_vote(const float* cls_prob_dev, const float* pred_boxes_dev, const int* num_rois_dev, int r, int batch,
+                                int num_classes, float score_thresh, int method, float sigma, float nt, float prune_thresh,
+                                int max_per_image, int max_det, float* det_dev, int* ndet_dev, int record_stride, int* keep_dev,
+                                int* keep_cnt_dev, float* keep_score_dev, void* workspace_dev, size_t workspace_bytes,
+                                float vote_thresh, int vote_method, float vote_beta, float* vote_box_dev, void* stream);
 /* per-detection head features, run after frcnn_detect_post on the same keep_dev / keep_cnt_dev: slot k of image b is record
  * row k of that image (classes ascending, slot = prefix(keep_cnt)[c] + j, slot < max_det).  fc7_dev [batch*r, feat_dim] is the
  * head output the class / box FC read (feat_dim % 4 == 0, 16-byte aligned).  roi_out_dev int32 [batch, max_det] = RoI index

@@ -18,6 +18,7 @@ ACT_NONE, ACT_RELU, ACT_RELU6 = 0, 1, 2
 CONV_F16X3, CONV_TF32X3, CONV_F16X1 = 0, 1, 2
 SOFT_NMS_METHODS = {"linear": 0, "gaussian": 1, "hard": 2}   # FRCNN_SOFT_NMS_*
 AUG_MAX_VIEWS = 16                                            # FRCNN_AUG_MAX_VIEWS
+BOX_VOTE_METHODS = {"ID": 0, "AVG": 1, "IOU_AVG": 2, "GENERALIZED_AVG": 3, "QUASI_SUM": 4, "TEMP_AVG": 5}   # FRCNN_BOX_VOTE_*
 
 vp, ci, cf, cu, sz = C.c_void_p, C.c_int, C.c_float, C.c_uint, C.c_size_t
 ip, fp = C.POINTER(C.c_int), C.POINTER(C.c_float)
@@ -73,6 +74,10 @@ SIGNATURES = {
     "frcnn_boxes_to_rois": (ci, [vp, vp, vp, ci, ci, vp, vp, vp]),
     "frcnn_preprocess_hflip": (ci, [vp, ci, ci, C.POINTER(C.c_double), C.c_double, C.c_double, vp, ci, ci, vp]),
     "frcnn_aug_union": (ci, [C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), ip, ip, ci, ci, ci, vp, vp, vp, vp, vp]),
+    "frcnn_box_vote_host": (ci, [fp, fp, ci, ci, fp, ci, ci, cf, ci, cf, ci]),
+    "frcnn_detect_post_vote": (ci, [vp, vp, vp, ci, ci, ci, cf, cf, cu, ci, ci, vp, vp, ci, vp, vp, vp, vp, sz, cf, ci, cf, vp, vp]),
+    "frcnn_detect_post_soft_vote": (ci, [vp, vp, vp, ci, ci, ci, cf, ci, cf, cf, cf, ci, ci, vp, vp, ci, vp, vp, vp, vp, sz, cf, ci, cf, vp,
+                                         vp]),
 }
 
 _lib = None

@@ -12,6 +12,8 @@
 // max_out boxes are kept, so the RPN stage touches only the first few thousand of the 17k-50k anchors.
 // IoU arithmetic is the oracle's op-by-op fp32 sequence (__f*_rn: no FMA contraction) for all three predicate
 // variants (flags), so survivor indices are bit-exact.
+#include <cfloat>
+
 #include "common.cuh"
 #include "../../include/frcnn_b200.h"
 
@@ -330,10 +332,12 @@ __device__ __forceinline__ int count_ge(const float* __restrict__ sorted_desc, i
   return lo;
 }
 
+// VOTED: the record box of keep entry (c, j) is vote_box[img][c][j] (box voting) instead of pred[keep[c][j]].
+template <bool VOTED>
 __global__ void __launch_bounds__(NMS_THREADS, 1)
 cap_emit_kernel(const float4* __restrict__ pred, int r, int C, int max_per_image, int max_det, int* __restrict__ keep,
                 int* __restrict__ keep_cnt, const float* __restrict__ keep_score, float* __restrict__ det, int* __restrict__ ndet,
-                int det_stride, int ndet_stride) {
+                int det_stride, int ndet_stride, const float4* __restrict__ vote_box) {
   __shared__ int s_warp[NMS_THREADS / 32];
   __shared__ int s_total;
   __shared__ int s_off[1025];
@@ -384,8 +388,9 @@ cap_emit_kernel(const float4* __restrict__ pred, int r, int C, int max_per_image
     if (j < keep_cnt[c]) {
       const int slot = s_off[c] + j;
       if (slot < max_det) {
-        const int roi = keep[(size_t)c * r + j];
-        const float4 b = __ldg(pred + (size_t)roi * C + c);
+        float4 b;
+        if (VOTED) b = __ldg(vote_box + ((size_t)img * C + c) * r + j);
+        else b = __ldg(pred + (size_t)keep[(size_t)c * r + j] * C + c);
         float* d = det + (size_t)slot * 6;
         d[0] = b.x; d[1] = b.y; d[2] = b.z; d[3] = b.w;
         d[4] = keep_score[(size_t)c * r + j]; d[5] = (float)c;
@@ -619,6 +624,167 @@ soft_nms_set_kernel(const float* __restrict__ dets, int n, int dim, SoftParams p
   if (threadIdx.x == 0) *num = nk;
 }
 
+// ---- box voting (Detectron's TEST.BBOX_VOTE) between the per-class stage and the cap ---------------------------------------
+// Definition and operation order: include/frcnn_b200.h (frcnn_box_vote_host).  The candidates are compacted into shared memory
+// in ascending input order (x1, y1, x2, y2, score arrays, compacted position p).  One warp votes one top box: lane l visits the
+// positions l, l+32, l+64, ... in ascending order and accumulates fp64 partials, then the xor butterfly 16, 8, 4, 2, 1 adds them
+// (IEEE addition commutes, so every lane ends with lane 0's bits), and lane 0 forms the outputs.  The fp32 products s*x, ov*s
+// and beta*s are exact in fp64, so an FMA contraction of an accumulation gives the same bits as a separate multiply and add.
+struct VoteParams { float thresh; int method; float beta; };
+
+constexpr size_t vote_smem_bytes(int cap) { return (size_t)cap * 24; }   // 5 candidate floats; the re-sort: float4 box | score | roi
+
+struct VoteAcc { double s, x1, y1, x2, y2, m0, m1; int n; };
+
+__device__ __forceinline__ void vote_add(VoteAcc& a, float4 t, float ta, float x1, float y1, float x2, float y2, float sc,
+                                         const VoteParams& p) {
+  const float iw = __fadd_rn(__fsub_rn(fminf(t.z, x2), fmaxf(t.x, x1)), 1.f);
+  if (!(iw > 0.f)) return;
+  const float ih = __fadd_rn(__fsub_rn(fminf(t.w, y2), fmaxf(t.y, y1)), 1.f);
+  if (!(ih > 0.f)) return;
+  const float inter = __fmul_rn(iw, ih);
+  const float ov = __fdiv_rn(inter, __fsub_rn(__fadd_rn(ta, area_plus1(x1, y1, x2, y2)), inter));
+  if (!(ov >= p.thresh)) return;
+  const double s = (double)sc;
+  a.s += s; a.x1 += s * (double)x1; a.y1 += s * (double)y1; a.x2 += s * (double)x2; a.y2 += s * (double)y2;
+  a.n += 1;
+  if (p.method == FRCNN_BOX_VOTE_IOU_AVG) {
+    a.m0 += (double)ov * s; a.m1 += (double)ov;
+  } else if (p.method == FRCNN_BOX_VOTE_GENERALIZED_AVG) {
+    a.m0 += exp((double)p.beta * s);
+  } else if (p.method == FRCNN_BOX_VOTE_TEMP_AVG) {
+    const double q = 1.0 - s, m = fmax(s, q), b = (double)p.beta;
+    const double e0 = exp(log(s / m) / b), e1 = exp(log(q / m) / b);
+    a.m0 += e0 / (e0 + e1);
+  }
+}
+
+__device__ __forceinline__ double xor_sum(double v) {
+#pragma unroll
+  for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// n^beta of QUASI_SUM: exact for beta 1 and 2 (n <= 8192), the correctly rounded sqrt for 0.5, else pow
+__device__ __forceinline__ double vote_pow(double n, double b) {
+  return b == 1.0 ? n : b == 2.0 ? n * n : b == 0.5 ? sqrt(n) : pow(n, b);
+}
+
+// The voted box and score of top box t (score ts) from the reduced sums; an empty vote set keeps both, a zero weight sum the box.
+__device__ __forceinline__ void vote_finish(const VoteAcc& a, const VoteParams& p, float4& t, float& ts) {
+  if (a.n == 0) return;
+  if (a.s != 0.0) t = make_float4((float)(a.x1 / a.s), (float)(a.y1 / a.s), (float)(a.x2 / a.s), (float)(a.y2 / a.s));
+  const double n = (double)a.n, b = (double)p.beta;
+  switch (p.method) {
+    case FRCNN_BOX_VOTE_AVG: ts = (float)(a.s / n); break;
+    case FRCNN_BOX_VOTE_IOU_AVG: ts = (float)(a.m0 / a.m1); break;
+    case FRCNN_BOX_VOTE_GENERALIZED_AVG: ts = (float)(log(a.m0 / n) / b); break;
+    case FRCNN_BOX_VOTE_QUASI_SUM: ts = (float)(a.s / vote_pow(n, b)); break;
+    case FRCNN_BOX_VOTE_TEMP_AVG: ts = (float)(a.m0 / n); break;
+    default: break;                                                   // ID: the NMS / Soft-NMS score
+  }
+}
+
+// CTA-cooperative voting (blockDim.x == T): candidates are the inputs e < n (n <= T*PER) with is_cand(e), box(e) / score(e);
+// top(i, box, score) reads top box i < n_top; out(i, box, score) is called by one lane per top box.  sm: vote_smem_bytes(T*PER).
+template <int T, int PER, typename CandFn, typename BoxFn, typename ScoreFn, typename TopFn, typename OutFn>
+__device__ void block_vote(int n, CandFn is_cand, BoxFn box, ScoreFn score, int n_top, TopFn top, const VoteParams prm, OutFn out,
+                           float* sm) {
+  constexpr int CAP = T * PER;
+  __shared__ int s_cnt[PER * (T / 32)];
+  float* x1 = sm; float* y1 = sm + CAP; float* x2 = sm + 2 * CAP; float* y2 = sm + 3 * CAP; float* sc = sm + 4 * CAP;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  bool f[PER];
+  int ex[PER];
+  const int rows = (n + T - 1) / T;
+#pragma unroll
+  for (int k = 0; k < PER; ++k) { const int e = k * T + tid; f[k] = k < rows && e < n && is_cand(e); }
+  const int N = block_count_rows<T, PER>(f, ex, rows, s_cnt);
+#pragma unroll
+  for (int k = 0; k < PER; ++k) {
+    if (f[k]) {
+      const int e = k * T + tid, p = ex[k];
+      const float4 b = box(e);
+      x1[p] = b.x; y1[p] = b.y; x2[p] = b.z; y2[p] = b.w; sc[p] = score(e);
+    }
+  }
+  __syncthreads();
+  for (int i = warp; i < n_top; i += T / 32) {
+    float4 t; float ts;
+    top(i, t, ts);
+    const float ta = area_plus1(t.x, t.y, t.z, t.w);
+    VoteAcc a{0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0};
+    for (int p = lane; p < N; p += 32) vote_add(a, t, ta, x1[p], y1[p], x2[p], y2[p], sc[p], prm);
+    a.s = xor_sum(a.s); a.x1 = xor_sum(a.x1); a.y1 = xor_sum(a.y1); a.x2 = xor_sum(a.x2); a.y2 = xor_sum(a.y2);
+    if (prm.method == FRCNN_BOX_VOTE_IOU_AVG || prm.method == FRCNN_BOX_VOTE_GENERALIZED_AVG || prm.method == FRCNN_BOX_VOTE_TEMP_AVG)
+      a.m0 = xor_sum(a.m0);
+    if (prm.method == FRCNN_BOX_VOTE_IOU_AVG) a.m1 = xor_sum(a.m1);
+#pragma unroll
+    for (int o = 16; o; o >>= 1) a.n += __shfl_xor_sync(0xffffffffu, a.n, o);
+    if (lane == 0) {
+      vote_finish(a, prm, t, ts);
+      out(i, t, ts);
+    }
+  }
+}
+
+// one CTA per (foreground class, image), after the per-class stage: votes the class's kept list keep / keep_score [0, keep_cnt)
+// against the stage's candidates (score > score_thresh, ascending RoI order, original scores), writes vote_box, and for a
+// score-changing method overwrites keep_score and re-sorts keep / keep_score / vote_box stably by descending voted score.
+template <int T, int PER>
+__global__ void __launch_bounds__(T)
+class_vote_kernel(const float* __restrict__ probs, const float4* __restrict__ pred, const int* __restrict__ num_rois, int r, int C,
+                  float score_thresh, VoteParams prm, int* __restrict__ keep, const int* __restrict__ keep_cnt,
+                  float* __restrict__ keep_score, float4* __restrict__ vote_box) {
+  constexpr int CAP = T * PER;
+  extern __shared__ __align__(16) float vote_dyn[];
+  const int cls = blockIdx.x + 1, img = blockIdx.y, tid = threadIdx.x;
+  probs += (size_t)img * r * C; pred += (size_t)img * r * C;
+  const size_t row = ((size_t)img * C + cls) * r;
+  int* ck = keep + row;
+  float* cs = keep_score + row;
+  float4* vb = vote_box + row;
+  const int nr = min(__ldg(num_rois + img), r);
+  const int nk = __ldg(keep_cnt + (size_t)img * C + cls);
+  const bool rescore = prm.method != FRCNN_BOX_VOTE_ID;
+  block_vote<T, PER>(
+      nr, [&](int e) { return __ldg(probs + (size_t)e * C + cls) > score_thresh; },
+      [&](int e) { return __ldg(pred + (size_t)e * C + cls); }, [&](int e) { return __ldg(probs + (size_t)e * C + cls); }, nk,
+      [&](int i, float4& b, float& s) { b = __ldg(pred + (size_t)ck[i] * C + cls); s = cs[i]; }, prm,
+      [&](int i, float4 b, float s) { vb[i] = b; if (rescore) cs[i] = s; }, vote_dyn);
+  if (!rescore) return;
+  // stable re-sort by descending voted score: rank = #(higher) + #(equal and earlier).  Voted scores are >= +0, so the order
+  // of their bit patterns is the float order, and a strict total order: the ranks are a permutation whatever the values.
+  __syncthreads();                                             // votes written; the candidate arrays are free
+  float4* sbox = reinterpret_cast<float4*>(vote_dyn);
+  unsigned* sbits = reinterpret_cast<unsigned*>(vote_dyn + 4 * CAP);
+  int* sroi = reinterpret_cast<int*>(vote_dyn + 5 * CAP);
+  for (int i = tid; i < nk; i += T) { sbox[i] = vb[i]; sbits[i] = __float_as_uint(cs[i]); sroi[i] = ck[i]; }
+  __syncthreads();
+  for (int i = tid; i < nk; i += T) {
+    const unsigned u = sbits[i];
+    int rank = 0;
+    for (int j = 0; j < nk; ++j) { const unsigned v = sbits[j]; rank += (v > u) | ((v == u) & (j < i)); }
+    vb[rank] = sbox[i]; cs[rank] = __uint_as_float(u); ck[rank] = sroi[i];
+  }
+}
+
+// one CTA: top rows [n_top, top_dim >= 5] voted against all rows [n_all, all_dim >= 5]; out [n_top, 5] in top's row order
+template <int T, int PER>
+__global__ void __launch_bounds__(T)
+box_vote_set_kernel(const float* __restrict__ top, int n_top, int top_dim, const float* __restrict__ all, int n_all, int all_dim,
+                    VoteParams prm, float* __restrict__ out) {
+  extern __shared__ __align__(16) float vote_dyn[];
+  block_vote<T, PER>(
+      n_all, [](int) { return true; },
+      [&](int e) { const float* d = all + (size_t)e * all_dim; return make_float4(d[0], d[1], d[2], d[3]); },
+      [&](int e) { return all[(size_t)e * all_dim + 4]; }, n_top,
+      [&](int i, float4& b, float& s) { const float* d = top + (size_t)i * top_dim; b = make_float4(d[0], d[1], d[2], d[3]); s = d[4]; },
+      prm,
+      [&](int i, float4 b, float s) { float* o = out + (size_t)i * 5; o[0] = b.x; o[1] = b.y; o[2] = b.z; o[3] = b.w; o[4] = s; },
+      vote_dyn);
+}
+
 // ---- per-detection head features ---------------------------------------------------------------------------
 // Runs after cap_emit_kernel and rebuilds its slot order from the truncated keep lists (classes ascending, slot =
 // prefix(keep_cnt)[c] + j), so slot k of the features is record row k.  One CTA per (block of FEAT_SLOTS slots, image):
@@ -787,32 +953,65 @@ static int smem_attr_once(K kernel, size_t bytes, bool (&done)[MAX_DEVICES]) {
   return OK;
 }
 
-// Both post entries: the shared checks, then class_stage(grid, st, pred) (its own checks, then the per-class launch), then the cap
-// and the records: image b's count at ndet[b*s], its rows at det + b*s, s = record_stride (0: det [batch, max_det, 6], ndet [batch]).
+static int vote_params(float thresh, int method, float beta, VoteParams* p, const char* who) {
+  FRCNN_REQUIRE(method >= FRCNN_BOX_VOTE_ID && method <= FRCNN_BOX_VOTE_TEMP_AVG,
+                "%s: method %d is not one of FRCNN_BOX_VOTE_ID ... FRCNN_BOX_VOTE_TEMP_AVG", who, method);
+  FRCNN_REQUIRE(thresh > 0.f && thresh <= 1.f, "%s: the vote threshold must lie in (0, 1]", who);
+  FRCNN_REQUIRE(beta > 0.f && beta <= FLT_MAX, "%s: beta must be finite and > 0", who);
+  *p = VoteParams{thresh, method, beta};
+  return OK;
+}
+
+// Both post entries: the shared checks, then class_stage(grid, st, pred) (its own checks, then the per-class launch), with `vote`
+// the box-voting stage into vote_box, then the cap and the records: image b's count at ndet[b*s], its rows at det + b*s,
+// s = record_stride (0: det [batch, max_det, 6], ndet [batch]).
 template <typename ClassStage>
 static int detect_post_run(const char* who, const float* cls_prob, const float* pred_boxes, const int* num_rois, int r, int batch,
-                           int num_classes, int max_per_image, int max_det, float* det, int* ndet, int record_stride, int* keep,
-                           int* keep_cnt, float* keep_score, void* stream, ClassStage class_stage) {
+                           int num_classes, float score_thresh, int max_per_image, int max_det, float* det, int* ndet, int record_stride,
+                           int* keep, int* keep_cnt, float* keep_score, const VoteParams* vote, float* vote_box, void* stream,
+                           ClassStage class_stage) {
   FRCNN_REQUIRE(cls_prob && pred_boxes && num_rois && det && ndet && keep && keep_cnt && keep_score, "%s: null pointer", who);
   FRCNN_REQUIRE(r > 0 && batch > 0 && num_classes >= 2 && num_classes <= 1024, "%s: r>0, batch>0, 2<=C<=1024 required", who);
   if (r > DET_CAP_BIG) { set_error("%s: %d RoIs per image > capacity %d", who, r, DET_CAP_BIG); return ERR_CAPACITY; }
   FRCNN_REQUIRE(record_stride == 0 || record_stride >= max_det * 6, "%s: record_stride %d < max_det*6", who, record_stride);
+  FRCNN_REQUIRE(!vote || (vote_box && ((uintptr_t)vote_box & 15) == 0), "%s: vote_box must be a 16-byte aligned device buffer", who);
   cudaStream_t st = (cudaStream_t)stream;
   const float4* pred = reinterpret_cast<const float4*>(pred_boxes);
-  if (int rc = class_stage(dim3((unsigned)(num_classes - 1), (unsigned)batch), st, pred)) return rc;
+  const dim3 grid((unsigned)(num_classes - 1), (unsigned)batch);
+  if (int rc = class_stage(grid, st, pred)) return rc;
   FRCNN_LAUNCH_CHECK();
-  cap_emit_kernel<<<(unsigned)batch, NMS_THREADS, 0, st>>>(pred, r, num_classes, max_per_image, max_det, keep, keep_cnt, keep_score, det, ndet,
-                                                          record_stride ? record_stride : max_det * 6, record_stride ? record_stride : 1);
+  const int rs = record_stride ? record_stride : max_det * 6, ns = record_stride ? record_stride : 1;
+  if (!vote) {
+    cap_emit_kernel<false><<<(unsigned)batch, NMS_THREADS, 0, st>>>(pred, r, num_classes, max_per_image, max_det, keep, keep_cnt,
+                                                                   keep_score, det, ndet, rs, ns, nullptr);
+    FRCNN_LAUNCH_CHECK();
+    return OK;
+  }
+  float4* vb = reinterpret_cast<float4*>(vote_box);
+  if (r <= DET_CAP) {
+    class_vote_kernel<SOFT_THREADS, SOFT_PER><<<grid, SOFT_THREADS, vote_smem_bytes(DET_CAP), st>>>(
+        cls_prob, pred, num_rois, r, num_classes, score_thresh, *vote, keep, keep_cnt, keep_score, vb);
+  } else {
+    static bool attr_done[MAX_DEVICES];
+    if (int rc = smem_attr_once(class_vote_kernel<SOFT_THREADS_BIG, SOFT_PER_BIG>, vote_smem_bytes(DET_CAP_BIG), attr_done)) return rc;
+    class_vote_kernel<SOFT_THREADS_BIG, SOFT_PER_BIG><<<grid, SOFT_THREADS_BIG, vote_smem_bytes(DET_CAP_BIG), st>>>(
+        cls_prob, pred, num_rois, r, num_classes, score_thresh, *vote, keep, keep_cnt, keep_score, vb);
+  }
+  FRCNN_LAUNCH_CHECK();
+  cap_emit_kernel<true><<<(unsigned)batch, NMS_THREADS, 0, st>>>(pred, r, num_classes, max_per_image, max_det, keep, keep_cnt, keep_score,
+                                                                det, ndet, rs, ns, vb);
   FRCNN_LAUNCH_CHECK();
   return OK;
 }
 
-extern "C" int frcnn_detect_post(const float* cls_prob, const float* pred_boxes, const int* num_rois, int r, int batch, int num_classes,
-                                 float score_thresh, float nms_thresh, unsigned flags, int max_per_image, int max_det,
-                                 float* det, int* ndet, int record_stride, int* keep, int* keep_cnt, float* keep_score, void* workspace,
-                                 size_t workspace_bytes, void* stream) {
-  return detect_post_run("detect_post", cls_prob, pred_boxes, num_rois, r, batch, num_classes, max_per_image, max_det, det, ndet,
-                         record_stride, keep, keep_cnt, keep_score, stream, [&](dim3 grid, cudaStream_t st, const float4* pred) -> int {
+// the greedy post (frcnn_detect_post / _vote); vote == nullptr: no voting stage
+static int greedy_post(const char* who, const float* cls_prob, const float* pred_boxes, const int* num_rois, int r, int batch,
+                       int num_classes, float score_thresh, float nms_thresh, unsigned flags, int max_per_image, int max_det, float* det,
+                       int* ndet, int record_stride, int* keep, int* keep_cnt, float* keep_score, void* workspace, size_t workspace_bytes,
+                       const VoteParams* vote, float* vote_box, void* stream) {
+  return detect_post_run(who, cls_prob, pred_boxes, num_rois, r, batch, num_classes, score_thresh, max_per_image, max_det, det,
+                         ndet, record_stride, keep, keep_cnt, keep_score, vote, vote_box, stream,
+                         [&](dim3 grid, cudaStream_t st, const float4* pred) -> int {
     if (r <= DET_CAP) {
       class_nms_kernel<DET_CAP, false><<<grid, NMS_THREADS, DET_CAP * 32, st>>>(cls_prob, pred, num_rois, r, num_classes, score_thresh,
                                                                                 nms_thresh, flags, keep, keep_cnt, keep_score, nullptr);
@@ -828,15 +1027,16 @@ extern "C" int frcnn_detect_post(const float* cls_prob, const float* pred_boxes,
   });
 }
 
-extern "C" int frcnn_detect_post_soft(const float* cls_prob, const float* pred_boxes, const int* num_rois, int r, int batch,
-                                      int num_classes, float score_thresh, int method, float sigma, float nt, float prune_thresh,
-                                      int max_per_image, int max_det, float* det, int* ndet, int record_stride, int* keep,
-                                      int* keep_cnt, float* keep_score, void* workspace, size_t workspace_bytes, void* stream) {
-  (void)workspace; (void)workspace_bytes;
-  return detect_post_run("detect_post_soft", cls_prob, pred_boxes, num_rois, r, batch, num_classes, max_per_image, max_det, det, ndet,
-                         record_stride, keep, keep_cnt, keep_score, stream, [&](dim3 grid, cudaStream_t st, const float4* pred) -> int {
+// the Soft-NMS post (frcnn_detect_post_soft / _soft_vote); vote == nullptr: no voting stage
+static int soft_post(const char* who, const float* cls_prob, const float* pred_boxes, const int* num_rois, int r, int batch, int num_classes,
+                     float score_thresh, int method, float sigma, float nt, float prune_thresh, int max_per_image, int max_det, float* det,
+                     int* ndet, int record_stride, int* keep, int* keep_cnt, float* keep_score, const VoteParams* vote, float* vote_box,
+                     void* stream) {
+  return detect_post_run(who, cls_prob, pred_boxes, num_rois, r, batch, num_classes, score_thresh, max_per_image, max_det, det, ndet,
+                         record_stride, keep, keep_cnt, keep_score, vote, vote_box, stream,
+                         [&](dim3 grid, cudaStream_t st, const float4* pred) -> int {
     SoftParams prm;
-    if (int rc = soft_params(method, sigma, nt, prune_thresh, &prm, "detect_post_soft")) return rc;
+    if (int rc = soft_params(method, sigma, nt, prune_thresh, &prm, who)) return rc;
     if (r <= DET_CAP) {
       class_soft_nms_kernel<SOFT_THREADS, SOFT_PER><<<grid, SOFT_THREADS, soft_smem_bytes(DET_CAP), st>>>(
           cls_prob, pred, num_rois, r, num_classes, score_thresh, prm, keep, keep_cnt, keep_score);
@@ -848,6 +1048,90 @@ extern "C" int frcnn_detect_post_soft(const float* cls_prob, const float* pred_b
         cls_prob, pred, num_rois, r, num_classes, score_thresh, prm, keep, keep_cnt, keep_score);
     return OK;
   });
+}
+
+extern "C" int frcnn_detect_post(const float* cls_prob, const float* pred_boxes, const int* num_rois, int r, int batch, int num_classes,
+                                 float score_thresh, float nms_thresh, unsigned flags, int max_per_image, int max_det,
+                                 float* det, int* ndet, int record_stride, int* keep, int* keep_cnt, float* keep_score, void* workspace,
+                                 size_t workspace_bytes, void* stream) {
+  return greedy_post("detect_post", cls_prob, pred_boxes, num_rois, r, batch, num_classes, score_thresh, nms_thresh, flags, max_per_image,
+                     max_det, det, ndet, record_stride, keep, keep_cnt, keep_score, workspace, workspace_bytes, nullptr, nullptr, stream);
+}
+
+extern "C" int frcnn_detect_post_vote(const float* cls_prob, const float* pred_boxes, const int* num_rois, int r, int batch,
+                                      int num_classes, float score_thresh, float nms_thresh, unsigned flags, int max_per_image, int max_det,
+                                      float* det, int* ndet, int record_stride, int* keep, int* keep_cnt, float* keep_score,
+                                      void* workspace, size_t workspace_bytes, float vote_thresh, int vote_method, float vote_beta,
+                                      float* vote_box, void* stream) {
+  VoteParams vp;
+  if (int rc = vote_params(vote_thresh, vote_method, vote_beta, &vp, "detect_post_vote")) return rc;
+  return greedy_post("detect_post_vote", cls_prob, pred_boxes, num_rois, r, batch, num_classes, score_thresh, nms_thresh, flags,
+                     max_per_image, max_det, det, ndet, record_stride, keep, keep_cnt, keep_score, workspace, workspace_bytes, &vp,
+                     vote_box, stream);
+}
+
+extern "C" int frcnn_detect_post_soft(const float* cls_prob, const float* pred_boxes, const int* num_rois, int r, int batch,
+                                      int num_classes, float score_thresh, int method, float sigma, float nt, float prune_thresh,
+                                      int max_per_image, int max_det, float* det, int* ndet, int record_stride, int* keep,
+                                      int* keep_cnt, float* keep_score, void* workspace, size_t workspace_bytes, void* stream) {
+  (void)workspace; (void)workspace_bytes;
+  return soft_post("detect_post_soft", cls_prob, pred_boxes, num_rois, r, batch, num_classes, score_thresh, method, sigma, nt, prune_thresh,
+                   max_per_image, max_det, det, ndet, record_stride, keep, keep_cnt, keep_score, nullptr, nullptr, stream);
+}
+
+extern "C" int frcnn_detect_post_soft_vote(const float* cls_prob, const float* pred_boxes, const int* num_rois, int r, int batch,
+                                           int num_classes, float score_thresh, int method, float sigma, float nt, float prune_thresh,
+                                           int max_per_image, int max_det, float* det, int* ndet, int record_stride, int* keep,
+                                           int* keep_cnt, float* keep_score, void* workspace, size_t workspace_bytes, float vote_thresh,
+                                           int vote_method, float vote_beta, float* vote_box, void* stream) {
+  (void)workspace; (void)workspace_bytes;
+  VoteParams vp;
+  if (int rc = vote_params(vote_thresh, vote_method, vote_beta, &vp, "detect_post_soft_vote")) return rc;
+  return soft_post("detect_post_soft_vote", cls_prob, pred_boxes, num_rois, r, batch, num_classes, score_thresh, method, sigma, nt,
+                   prune_thresh, max_per_image, max_det, det, ndet, record_stride, keep, keep_cnt, keep_score, &vp, vote_box, stream);
+}
+
+extern "C" int frcnn_box_vote_host(float* dets_out, const float* top_host, int n_top, int top_dim, const float* all_host, int n_all,
+                                   int all_dim, float thresh, int method, float beta, int device_id) {
+  FRCNN_REQUIRE(dets_out, "box_vote_host: null output");
+  VoteParams prm;
+  int rc = vote_params(thresh, method, beta, &prm, "box_vote_host");
+  if (rc) return rc;
+  if (n_top <= 0) return OK;
+  FRCNN_REQUIRE(top_host && top_dim >= 5, "box_vote_host: bad top rows (rows of >= 5 floats: x1, y1, x2, y2, score)");
+  if (n_all < 0) n_all = 0;
+  FRCNN_REQUIRE(n_all == 0 || (all_host && all_dim >= 5), "box_vote_host: bad candidate rows (rows of >= 5 floats: x1, y1, x2, y2, score)");
+  if (n_all > DET_CAP_BIG) { set_error("box_vote_host: %d candidates > capacity %d", n_all, DET_CAP_BIG); return ERR_CAPACITY; }
+  int cur = -1;
+  FRCNN_CUDA(cudaGetDevice(&cur));
+  const int dev = device_id < 0 ? cur : device_id;
+  if (cur != dev) FRCNN_CUDA(cudaSetDevice(dev));
+  static bool attr_done[MAX_DEVICES];
+  if (n_all > DET_CAP) rc = smem_attr_once(box_vote_set_kernel<SOFT_THREADS_BIG, SOFT_PER_BIG>, vote_smem_bytes(DET_CAP_BIG), attr_done);
+  float* dtop = nullptr; float* dall = nullptr; float* dout = nullptr;
+  cudaError_t e = cudaSuccess;
+  if (!rc) {
+    e = cudaMalloc(&dtop, (size_t)n_top * top_dim * sizeof(float));
+    if (e == cudaSuccess) e = cudaMalloc(&dout, (size_t)n_top * 5 * sizeof(float));
+    if (e == cudaSuccess && n_all > 0) e = cudaMalloc(&dall, (size_t)n_all * all_dim * sizeof(float));
+    if (e == cudaSuccess) e = cudaMemcpy(dtop, top_host, (size_t)n_top * top_dim * sizeof(float), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && n_all > 0) e = cudaMemcpy(dall, all_host, (size_t)n_all * all_dim * sizeof(float), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) {
+      if (n_all <= DET_CAP)
+        box_vote_set_kernel<SOFT_THREADS, SOFT_PER><<<1, SOFT_THREADS, vote_smem_bytes(DET_CAP)>>>(dtop, n_top, top_dim, dall, n_all,
+                                                                                                  all_dim, prm, dout);
+      else
+        box_vote_set_kernel<SOFT_THREADS_BIG, SOFT_PER_BIG><<<1, SOFT_THREADS_BIG, vote_smem_bytes(DET_CAP_BIG)>>>(
+            dtop, n_top, top_dim, dall, n_all, all_dim, prm, dout);
+      e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpy(dets_out, dout, (size_t)n_top * 5 * sizeof(float), cudaMemcpyDeviceToHost);
+    cudaFree(dtop); cudaFree(dall); cudaFree(dout);
+  }
+  if (cur != dev) cudaSetDevice(cur);                    // leave the caller's (torch's) current device untouched
+  if (rc) return rc;
+  if (e != cudaSuccess) return cuda_fail(e, "frcnn_box_vote_host", __FILE__, __LINE__);
+  return OK;
 }
 
 extern "C" int frcnn_soft_nms_host(float* dets_out, int* keep_out, int* num_out, const float* dets_host, int n, int dim, int method,

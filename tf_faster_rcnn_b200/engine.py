@@ -199,14 +199,16 @@ class Tape:
 
 REC_HEADER = 8     # 4-byte words in front of every image's detection rows: word 0 = int32 detection count
 
-# the options the post step is built for; a change rebuilds it (PostStage._ensure_post).  soft_nms: soft_nms_args() or None
-PostKey = collections.namedtuple("PostKey", "score_thresh nms_thresh use_gpu_nms max_per_image soft_nms")
+# the options the post step is built for; a change rebuilds it (PostStage._ensure_post).  soft_nms: soft_nms_args() or None;
+# box_vote: box_vote_args() or None
+PostKey = collections.namedtuple("PostKey", "score_thresh nms_thresh use_gpu_nms max_per_image soft_nms box_vote", defaults=(None,))
 
 
 class PostStage:
     """The test_net tail of a plan whose im_detect outputs are `cls_prob`, `pred_boxes` and `num_rois` (`batch` images of `R`
-    rows): the per-class NMS or Soft-NMS into `keep` / `keep_cnt` / `keep_score` (`post_ws`: the greedy NMS's workspace), the
-    max_per_image cap and the detection records, built on first use for the options in force; in feature mode also the
+    rows): the per-class NMS or Soft-NMS into `keep` / `keep_cnt` / `keep_score` (`post_ws`: the greedy NMS's workspace), with
+    the box_vote option the voting into `vote_box`, the max_per_image cap and the detection records, built on first use for the
+    options in force; in feature mode also the
     per-detection gather of `fc7`.  The subclass allocates those buffers.  Two record buffers: with `double_buffer`,
     consecutive detect launches alternate between them.  Also the plan's CUDA-graph cache."""
 
@@ -217,6 +219,7 @@ class PostStage:
         self.rec = self.ndet = None    # views of the buffer the LAST detect launch wrote
         self.post_steps = [None, None]
         self.feat_out = self.roi_out = self.features_step = None   # feature mode (_ensure_post(features=True))
+        self.vote_box = None                                        # box voting (_build_post)
         self.double_buffer = False
         self.slot = 0
         self.max_det = 0
@@ -224,12 +227,12 @@ class PostStage:
         self.use_graph = use_graph
 
     def _ensure_post(self, features=False):
-        """(Re)build the detection-record buffers and the post step for the current score / NMS thresholds, cap and Soft-NMS
-        setting; with `features`, also the per-detection feature buffers and their gather step."""
+        """(Re)build the detection-record buffers and the post step for the current score / NMS thresholds, cap, Soft-NMS and
+        box-voting settings; with `features`, also the per-detection feature buffers and their gather step."""
         o = self.net.options
-        soft = o.get("soft_nms")
+        soft, vote = o.get("soft_nms"), o.get("box_vote")
         key = PostKey(float(o["score_thresh"]), float(o["nms_thresh"]), bool(o["use_gpu_nms"]), int(o["max_per_image"]),
-                      None if soft is None else soft_nms_args(*soft))
+                      None if soft is None else soft_nms_args(*soft), None if vote is None else box_vote_args(*vote))
         if key != self.post_key:
             self._build_post(key)
         if features and self.features_step is None:
@@ -247,6 +250,9 @@ class PostStage:
         # A record set that still does not fit is reported through ndet > max_det and raised on the host (never truncated).
         self.max_det = max_det = 2 * mpi + 56 if mpi > 0 else R * (C - 1)
         thr, flags = nms_threshold(key.nms_thresh, key.use_gpu_nms)
+        # box voting: the voted boxes [B, C, R] float4 the records read (allocated only with the option on)
+        self.vote_box = None if key.box_vote is None else ops.zeros((B, C, R, 4))
+        vote = None if key.box_vote is None else (*key.box_vote, self.vote_box)
 
         def make_post(rec):
             # as_strided: view() repacks a size-1 batch dimension, which would drop the record stride at batch 1
@@ -254,9 +260,9 @@ class PostStage:
             if soft is not None:
                 return lambda: ops.detect_post_soft(self.cls_prob, self.pred_boxes, self.num_rois, C, key.score_thresh, soft[0], soft[1],
                                                     float(F(key.nms_thresh)), soft[2], mpi, det, ndet, self.keep, self.keep_cnt,
-                                                    self.keep_score, batch=B)
+                                                    self.keep_score, batch=B, vote=vote)
             return lambda: ops.detect_post(self.cls_prob, self.pred_boxes, self.num_rois, C, key.score_thresh, thr, flags, mpi, det, ndet,
-                                           self.keep, self.keep_cnt, self.keep_score, self.post_ws, batch=B)
+                                           self.keep, self.keep_cnt, self.keep_score, self.post_ws, batch=B, vote=vote)
         self.recs = [ops.zeros((B, REC_HEADER + max_det * 6)) for _ in range(2)]
         self.post_steps = [make_post(r) for r in self.recs]
         self.post_key = key
@@ -675,6 +681,26 @@ def soft_nms_option(node):
         return None
     soft_nms_args(node["METHOD"], node["SIGMA"], node["SCORE_THRESH"])
     return (node["METHOD"], float(node["SIGMA"]), float(node["SCORE_THRESH"]))
+
+
+def box_vote_args(vote_th, scoring_method="ID", beta=1.0):
+    """Box-voting parameters -> (fp32 VOTE_TH, FRCNN_BOX_VOTE_* code, fp32 beta); raises ValueError before any device work."""
+    if scoring_method not in N.BOX_VOTE_METHODS:
+        raise ValueError("box voting SCORING_METHOD %r: expected one of %s" % (scoring_method, ", ".join(N.BOX_VOTE_METHODS)))
+    t32, b32 = F(vote_th), F(beta)
+    if not 0 < t32 <= 1:
+        raise ValueError("box voting VOTE_TH must lie in (0, 1], got %r" % (vote_th,))
+    if not (np.isfinite(b32) and b32 > 0):
+        raise ValueError("box voting SCORING_METHOD_BETA must be finite and > 0, got %r" % (beta,))
+    return float(t32), N.BOX_VOTE_METHODS[scoring_method], float(b32)
+
+
+def box_vote_option(node):
+    """cfg.TEST.BBOX_VOTE -> the network option: None when disabled, else the checked (VOTE_TH, SCORING_METHOD, SCORING_METHOD_BETA)."""
+    if not node["ENABLED"]:
+        return None
+    box_vote_args(node["VOTE_TH"], node["SCORING_METHOD"], node["SCORING_METHOD_BETA"])
+    return (float(node["VOTE_TH"]), node["SCORING_METHOD"], float(node["SCORING_METHOD_BETA"]))
 
 
 def nms_threshold(thresh, use_gpu_nms):

@@ -60,6 +60,10 @@ cfg = AttrDict(
         # BBOX_AUG.SCALES entry (short side, long side capped by BBOX_AUG.MAX_SIZE), and with H_FLIP the mirrored twin of each; the
         # boxes of every view are merged ahead of the per-class NMS (model/test.py::aug_views gives the order)
         BBOX_AUG=dict(ENABLED=False, H_FLIP=False, SCALES=(), MAX_SIZE=2000),
+        # extension (Detectron's TEST.BBOX_VOTE): after the per-class NMS / Soft-NMS each kept box becomes the score-weighted mean
+        # of its class's candidates overlapping it by >= VOTE_TH (0 < VOTE_TH <= 1); SCORING_METHOD ID (score unchanged) | AVG |
+        # IOU_AVG | GENERALIZED_AVG | QUASI_SUM | TEMP_AVG, SCORING_METHOD_BETA finite and > 0.  The max_per_image cap follows.
+        BBOX_VOTE=dict(ENABLED=False, VOTE_TH=0.8, SCORING_METHOD="ID", SCORING_METHOD_BETA=1.0),
     ),
     RESNET=dict(MAX_POOL=False, FIXED_BLOCKS=1),
     MOBILENET=dict(REGU_DEPTH=False, FIXED_LAYERS=5, WEIGHT_DECAY=0.00004, DEPTH_MULTIPLIER=1.0),

@@ -17,7 +17,7 @@ import numpy as np
 import torch
 
 from model.config import cfg, get_output_dir
-from model.nms_wrapper import nms, soft_nms
+from model.nms_wrapper import box_voting, nms, soft_nms
 from tf_faster_rcnn_b200 import engine
 from utils.blob import im_list_to_blob
 from utils.timer import Timer
@@ -200,18 +200,24 @@ def apply_nms(all_boxes, thresh):
 
 
 def _detections_python_loop(scores, boxes, num_classes, thresh, max_per_image):
-    """test.py:162-180 verbatim flow over the (GPU) nms(), or soft_nms() per class when TEST.SOFT_NMS.ENABLED."""
+    """test.py:162-180 verbatim flow over the (GPU) nms(), or soft_nms() per class when TEST.SOFT_NMS.ENABLED; with
+    TEST.BBOX_VOTE.ENABLED each class's kept rows are then voted against its candidates (box_voting) and, for a score-changing
+    method, re-sorted stably by descending voted score, as the fused post does."""
     per_class = [np.zeros((0, 5), np.float32)]
+    bv = cfg.TEST.BBOX_VOTE
     for j in range(1, num_classes):
         inds = np.where(scores[:, j] > thresh)[0]
         cls_dets = np.hstack((boxes[inds, j * 4:(j + 1) * 4], scores[inds, j][:, np.newaxis])).astype(np.float32, copy=False)
         if cfg.TEST.SOFT_NMS.ENABLED:
             sn = cfg.TEST.SOFT_NMS
             kept, _ = soft_nms(cls_dets, sn.SIGMA, cfg.TEST.NMS, sn.SCORE_THRESH, sn.METHOD)
-            per_class.append(kept)
-            continue
-        keep = nms(cls_dets, cfg.TEST.NMS)
-        per_class.append(cls_dets[keep, :])
+        else:
+            kept = cls_dets[nms(cls_dets, cfg.TEST.NMS), :]
+        if bv.ENABLED:
+            kept = box_voting(kept, cls_dets, bv.VOTE_TH, bv.SCORING_METHOD, bv.SCORING_METHOD_BETA)
+            if bv.SCORING_METHOD != "ID":
+                kept = kept[np.argsort(-kept[:, 4], kind="stable")]
+        per_class.append(kept)
     if max_per_image > 0:
         image_scores = np.hstack([d[:, -1] for d in per_class[1:]])
         if len(image_scores) > max_per_image:
@@ -239,6 +245,7 @@ def _set_post_options(net, thresh, max_per_image):
     net.options["score_thresh"], net.options["max_per_image"] = float(thresh), int(max_per_image)
     net.options["nms_thresh"] = cfg.TEST.NMS
     net.options["soft_nms"] = engine.soft_nms_option(cfg.TEST.SOFT_NMS)
+    net.options["box_vote"] = engine.box_vote_option(cfg.TEST.BBOX_VOTE)
 
 
 def _detect_record(net, im, thresh, max_per_image):

@@ -54,7 +54,7 @@ class Network(object):
             pooling_size=cfg.POOLING_SIZE, resnet_max_pool=bool(cfg.RESNET.MAX_POOL),
             bbox_stds=tuple(cfg.TRAIN.BBOX_NORMALIZE_STDS), bbox_means=tuple(cfg.TRAIN.BBOX_NORMALIZE_MEANS),
             nms_thresh=cfg.TEST.NMS, max_per_image=100, score_thresh=0.0, rpn_channels=cfg.RPN_CHANNELS,
-            soft_nms=engine.soft_nms_option(cfg.TEST.SOFT_NMS),
+            soft_nms=engine.soft_nms_option(cfg.TEST.SOFT_NMS), box_vote=engine.box_vote_option(cfg.TEST.BBOX_VOTE),
         )
         if self.options["test_mode"] not in ("nms", "top"):
             raise NotImplementedError

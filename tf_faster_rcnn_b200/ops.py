@@ -229,27 +229,43 @@ def _record_stride(det, ndet):
     return det.stride(0)
 
 
+def _vote_args(vote, keep):
+    """vote = (thresh, method, beta, vote_box): fp32 threshold, FRCNN_BOX_VOTE_* code, fp32 beta (engine.box_vote_args) and the
+    [batch, C, r, 4] fp32 buffer of the voted boxes -> the trailing C arguments of the _vote entries."""
+    thresh, method, beta, vote_box = vote
+    assert vote_box.dtype == torch.float32 and vote_box.is_contiguous() and vote_box.shape == (*keep.shape, 4), "vote_box [batch, C, r, 4]"
+    return float(thresh), int(method), float(beta), _p(vote_box)
+
+
 def detect_post(cls_prob, pred_boxes, num_rois, num_classes, score_thresh, nms_thresh, flags, max_per_image, det, ndet, keep,
-                keep_cnt, keep_score, workspace=None, batch=1):
+                keep_cnt, keep_score, workspace=None, batch=1, vote=None):
     """cls_prob [batch*r, C]; det [batch, max_det, 6] (or [max_det, 6] for batch 1); ndet int32 [batch] = TRUE counts
-    (a count above max_det means the records did not fit).  det and ndet may be views of record buffers (_record_stride)."""
+    (a count above max_det means the records did not fit).  det and ndet may be views of record buffers (_record_stride).
+    vote: None, or (thresh, method, beta, vote_box) for box voting ahead of the cap (frcnn_detect_post_vote)."""
     r = cls_prob.shape[0] // batch
     max_det = det.shape[-2]
-    N.check(N.lib().frcnn_detect_post(_p(cls_prob), _p(pred_boxes), _p(num_rois), r, batch, num_classes, float(score_thresh),
-                                      float(nms_thresh), flags, max_per_image, max_det, _p(det), _p(ndet), _record_stride(det, ndet),
-                                      _p(keep), _p(keep_cnt), _p(keep_score), _p(workspace), 0 if workspace is None else workspace.numel(),
-                                      _stream()), "detect_post")
+    args = (_p(cls_prob), _p(pred_boxes), _p(num_rois), r, batch, num_classes, float(score_thresh), float(nms_thresh), flags, max_per_image,
+            max_det, _p(det), _p(ndet), _record_stride(det, ndet), _p(keep), _p(keep_cnt), _p(keep_score), _p(workspace),
+            0 if workspace is None else workspace.numel())
+    if vote is None:
+        N.check(N.lib().frcnn_detect_post(*args, _stream()), "detect_post")
+    else:
+        N.check(N.lib().frcnn_detect_post_vote(*args, *_vote_args(vote, keep), _stream()), "detect_post_vote")
 
 
 def detect_post_soft(cls_prob, pred_boxes, num_rois, num_classes, score_thresh, method, sigma, nt, prune_thresh, max_per_image, det,
-                     ndet, keep, keep_cnt, keep_score, batch=1):
-    """detect_post with Soft-NMS as the per-class stage; method is an FRCNN_SOFT_NMS_* code (N.SOFT_NMS_METHODS)."""
+                     ndet, keep, keep_cnt, keep_score, batch=1, vote=None):
+    """detect_post with Soft-NMS as the per-class stage; method is an FRCNN_SOFT_NMS_* code (N.SOFT_NMS_METHODS).  vote: as for
+    detect_post (frcnn_detect_post_soft_vote)."""
     r = cls_prob.shape[0] // batch
     max_det = det.shape[-2]
-    N.check(N.lib().frcnn_detect_post_soft(_p(cls_prob), _p(pred_boxes), _p(num_rois), r, batch, num_classes, float(score_thresh),
-                                           int(method), float(sigma), float(nt), float(prune_thresh), max_per_image, max_det, _p(det),
-                                           _p(ndet), _record_stride(det, ndet), _p(keep), _p(keep_cnt), _p(keep_score), None, 0,
-                                           _stream()), "detect_post_soft")
+    args = (_p(cls_prob), _p(pred_boxes), _p(num_rois), r, batch, num_classes, float(score_thresh), int(method), float(sigma), float(nt),
+            float(prune_thresh), max_per_image, max_det, _p(det), _p(ndet), _record_stride(det, ndet), _p(keep), _p(keep_cnt),
+            _p(keep_score), None, 0)
+    if vote is None:
+        N.check(N.lib().frcnn_detect_post_soft(*args, _stream()), "detect_post_soft")
+    else:
+        N.check(N.lib().frcnn_detect_post_soft_vote(*args, *_vote_args(vote, keep), _stream()), "detect_post_soft_vote")
 
 
 def detect_features(keep, keep_cnt, fc7, num_classes, feat_out, roi_out):
@@ -309,3 +325,15 @@ def soft_nms_host(dets, method, sigma, nt, score_thresh, device_id=-1):
                                         d.shape[1] if n else 5, int(method), float(sigma), float(nt), float(score_thresh), device_id),
             "soft_nms_host")
     return out[:num.value].copy(), keep[:num.value].copy()
+
+
+def box_vote_host(top_dets, all_dets, thresh, method, beta, device_id=-1):
+    """Box voting of one set of HOST rows (x1, y1, x2, y2, score, ...): top_dets [n, >=5] voted against the candidates all_dets
+    [m, >=5]; method is an FRCNN_BOX_VOTE_* code.  -> fp32 [n, 5], the voted rows in top_dets' row order."""
+    t = np.ascontiguousarray(top_dets, dtype=np.float32)
+    a = np.ascontiguousarray(all_dets, dtype=np.float32)
+    n, m = t.shape[0], a.shape[0]
+    out = np.empty((max(n, 1), 5), dtype=np.float32)
+    N.check(N.lib().frcnn_box_vote_host(out.ctypes.data_as(N.fp), t.ctypes.data_as(N.fp), n, t.shape[1] if n else 5, a.ctypes.data_as(N.fp),
+                                        m, a.shape[1] if m else 5, float(thresh), int(method), float(beta), device_id), "box_vote_host")
+    return out[:n].copy()
