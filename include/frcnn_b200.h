@@ -231,7 +231,9 @@ int frcnn_detect_post(const float* cls_prob_dev, const float* pred_boxes_dev, co
  * being dropped.  An extension beyond the reference (Detectron's TEST.SOFT_NMS).  Per candidate list a[0..N) (each row
  * x1,y1,x2,y2,s):
  *   for i = 0, 1, ... while i < N:
- *     m = the lowest position in [i, N) holding the maximal score; swap a[i], a[m]; p = i + 1
+ *     m = i; for q = i+1 .. N-1: if a[m].s < a[q].s: m = q   (the lowest position of the maximal score; a NaN score at i is
+ *         selected at once, and otherwise NaN scores wait until only NaN scores are left)
+ *     swap a[i], a[m]; p = i + 1
  *     while p < N: decay a[p] by a[i]; if a[p] overlapped a[i] and its new score < score_thresh: a[p] = a[N-1], N -= 1
  *                  (position p is examined again) else p += 1
  *   result: a[0..N) in this order with the decayed scores.

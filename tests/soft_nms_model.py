@@ -8,6 +8,14 @@ F = np.float32
 METHODS = ("linear", "gaussian", "hard")
 
 
+def scan_argmax(s):
+    """Offset of the definition's selection in s: m = 0, then m = p wherever s[m] < s[p].  A NaN head is selected; otherwise
+    the first maximum of the non-NaN scores (np.argmax alone would take the first NaN anywhere)."""
+    if np.isnan(s[0]):
+        return 0
+    return int(np.argmax(np.where(np.isnan(s), -np.inf, s)))
+
+
 def soft_nms_model(dets, method="linear", sigma=0.5, nt=0.3, score_thresh=0.001):
     """dets [n,>=5] -> (rows [k,5] fp32 in selection order with decayed scores, keep [k] int32 rows of dets)."""
     assert method in METHODS
@@ -19,7 +27,7 @@ def soft_nms_model(dets, method="linear", sigma=0.5, nt=0.3, score_thresh=0.001)
     one = F(1)
     N, i = d.shape[0], 0
     while i < N:
-        m = i + int(np.argmax(s[i:N]))               # first (lowest) position of the maximum
+        m = i + scan_argmax(s[i:N])
         for c in cols:
             c[i], c[m] = c[m], c[i]
         L = i + 1

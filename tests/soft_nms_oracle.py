@@ -31,20 +31,26 @@ def lib():
         fp, ip = ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_int)
         L.oracle_soft_nms.argtypes = [fp, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_float, fp, ip]
         L.oracle_soft_nms.restype = ctypes.c_int
+        L.oracle_soft_nms_variant.argtypes = L.oracle_soft_nms.argtypes + [ctypes.c_int]
+        L.oracle_soft_nms_variant.restype = ctypes.c_int
         _LIB = L
     return _LIB
 
 
-def soft_nms_c(dets, method="linear", sigma=0.5, nt=0.3, score_thresh=0.001):
+# oracle variants: deliberate mistakes that the float64 comparator of post_ref64.py must catch
+GE_NT, NO_PLUS_ONE, PRUNE_UNTOUCHED, TIES_HIGH, STABLE_COMPACT, GAUSS_NO_SQUARE = 1, 2, 4, 8, 16, 32
+
+
+def soft_nms_c(dets, method="linear", sigma=0.5, nt=0.3, score_thresh=0.001, variant=0):
     """dets [n,>=5] -> (rows [k,5] fp32 in selection order with decayed scores, keep [k] int32 rows of dets).  Parameters are
     rounded to fp32 once, as the product does."""
     d = np.ascontiguousarray(np.asarray(dets, dtype=F)[:, :5])
     n = d.shape[0]
     out = np.zeros((max(n, 1), 5), F)
     keep = np.zeros(max(n, 1), np.int32)
-    k = lib().oracle_soft_nms(d.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), n, METHODS[method], float(F(sigma)), float(F(nt)),
-                              float(F(score_thresh)), out.ctypes.data_as(ctypes.POINTER(ctypes.c_float)),
-                              keep.ctypes.data_as(ctypes.POINTER(ctypes.c_int)))
+    k = lib().oracle_soft_nms_variant(d.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), n, METHODS[method], float(F(sigma)),
+                                      float(F(nt)), float(F(score_thresh)), out.ctypes.data_as(ctypes.POINTER(ctypes.c_float)),
+                                      keep.ctypes.data_as(ctypes.POINTER(ctypes.c_int)), int(variant))
     return out[:k].copy(), keep[:k].copy()
 
 

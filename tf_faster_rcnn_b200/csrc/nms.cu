@@ -472,6 +472,13 @@ __device__ __forceinline__ void better_of(float& s, int& pos, float s2, int p2) 
   if (s2 > s || (s2 == s && p2 < pos)) { s = s2; pos = p2; }
 }
 
+// The argmax key of score s at position p when `head` is the next selection's first position.  The definition's scan
+// (m = head; m = p where s[m] < s[p]) keeps a NaN head and never moves onto a NaN from a number: so a NaN at the head competes
+// as +inf (ties go to the lowest position, the head), and any other NaN never wins (better_of's comparisons are false).
+__device__ __forceinline__ float scan_key(float s, int p, int head) {
+  return (p == head && isnan(s)) ? __int_as_float(0x7f800000) : s;
+}
+
 // Position of the block's best (score, position): larger score first, then lower position.  One barrier; every thread gets
 // the result.  Threads without a candidate pass (-inf, 0x7fffffff).
 template <int T>
@@ -519,13 +526,13 @@ __device__ int block_soft_nms(int n, CandFn is_cand, BoxFn box, ScoreFn score, c
       const float4 b = box(e);
       const float s = score(e);
       x1[p] = b.x; y1[p] = b.y; x2[p] = b.z; y2[p] = b.w; sc[p] = s; id[p] = e;
-      better_of(bs, bp, s, p);
+      better_of(bs, bp, scan_key(s, p, 0), p);
     }
   }
   int m = block_argmax<T>(bs, bp, s_as, s_ap);
   for (int i = 0; i < N; ++i) {
-    // the selection sits at m; position m holds the former a[i] (the swap is applied lazily: its owner reads from i).  Only
-    // NaN scores can leave the argmax empty; the sequential scan then keeps position i.
+    // the selection sits at m; position m holds the former a[i] (the swap is applied lazily: its owner reads from i).  A NaN
+    // at position i entered the argmax as +inf (scan_key), so the argmax is never empty while i < N; the guard is defensive.
     if (m >= N) m = i;
     const float tx1 = x1[m], ty1 = y1[m], tx2 = x2[m], ty2 = y2[m];
     if (tid == 0) emit(i, id[m], make_float4(tx1, ty1, tx2, ty2), sc[m]);
@@ -557,7 +564,7 @@ __device__ int block_soft_nms(int n, CandFn is_cand, BoxFn box, ScoreFn score, c
         } else {                                    // survivor that keeps its position
           sc[p] = ns[k];
           if (p == m && m != i) { x1[p] = x1[i]; y1[p] = y1[i]; x2[p] = x2[i]; y2[p] = y2[i]; id[p] = id[i]; }
-          better_of(bs, bp, ns[k], p);
+          better_of(bs, bp, scan_key(ns[k], p, L), p);
         }
       }
     }
@@ -570,7 +577,7 @@ __device__ int block_soft_nms(int n, CandFn is_cand, BoxFn box, ScoreFn score, c
           const int dst = hole[(N - 1 - p) - (D - ex[k])];
           const int src = p == m ? i : p;
           x1[dst] = x1[src]; y1[dst] = y1[src]; x2[dst] = x2[src]; y2[dst] = y2[src]; id[dst] = id[src]; sc[dst] = ns[k];
-          better_of(bs, bp, ns[k], dst);
+          better_of(bs, bp, scan_key(ns[k], dst, L), dst);
         }
       }
     }
