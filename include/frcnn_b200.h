@@ -116,6 +116,16 @@ typedef struct {
   int split_k;               /* 0 = choose; 1 = never; n = split the K loop over n CTAs + deterministic reduce pass */
   int impl;                  /* FRCNN_CONV_F16X3 (0, default) | FRCNN_CONV_TF32X3 (kept for A/B measurements) | FRCNN_CONV_F16X1 */
   float out_mult;            /* F16X3: 2^-wexp of frcnn_pack_conv_weights (0 is read as 1) */
+  /* Second A source (pointwise layers only: 1x1, stride 1, no padding): K = cin + cin2, the packed weights are
+   * [cout][cin + cin2] and the input channels cin .. cin + cin2 - 1 are read from in2_dev [n, h, w, cin2].  A ResNet
+   * projection shortcut rides in the closing 1x1 conv's K loop this way.  NULL / 0 = one source. */
+  const float* in2_dev;
+  int cin2;                  /* 0, or a positive multiple of 32 */
+  /* Mean epilogue (pointwise layers only), on when mean_hw > 0: instead of out_dev, write mean_dev[p / mean_hw, cout] = the
+   * mean of the activated outputs of the mean_hw consecutive pixels p of each group (n*h*w % mean_hw == 0); out_dev is not
+   * written and may be NULL.  Summed in a fixed order (no atomics), divided once by mean_hw.  Never split along K. */
+  float* mean_dev;
+  int mean_hw;               /* 0 = off */
 } frcnn_conv_desc;
 
 int frcnn_conv_plan_create(frcnn_conv_plan** out, const frcnn_conv_desc* d);

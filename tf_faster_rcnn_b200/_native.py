@@ -30,7 +30,7 @@ class ConvDesc(C.Structure):
                 ("residual_dev", vp), ("out_dev", vp),
                 ("n", ci), ("h", ci), ("w", ci), ("cin", ci), ("cout", ci), ("kh", ci), ("kw", ci), ("stride", ci),
                 ("pad_t", ci), ("pad_l", ci), ("ho", ci), ("wo", ci), ("act", ci), ("block_n", ci), ("kb_per_chunk", ci), ("split_k", ci),
-                ("impl", ci), ("out_mult", cf)]
+                ("impl", ci), ("out_mult", cf), ("in2_dev", vp), ("cin2", ci), ("mean_dev", vp), ("mean_hw", ci)]
 
 
 # name -> (restype, argtypes); must list every symbol of include/frcnn_b200.h (checked by tests/test_abi.py)

@@ -75,6 +75,13 @@ struct ConvKernelParams {
   float* ws;
   long long* trace;   // debug: clock64() stamps of CTA 0's pipeline hand-offs; normally NULL
   int num_kb_total;   // k-blocks of the whole K loop (64 channels for the f16 modes, 32 for tf32)
+  int cin2;           // channels of the second A source (tmA2; pointwise layers only), 0 = none
+  // Mean epilogue (pointwise layers only, never split): tile mt's activated rows are summed per group of mean_hw pixels
+  // into mean_ws[mt][s][n_tiles*BN] (s = group - first group of the tile, s < mean_segs); mean_finish_kernel adds the
+  // partials of each group in tile order and divides by mean_hw into mean_out [pixels / mean_hw][cout].
+  float* mean_out;
+  float* mean_ws;
+  int mean_hw, mean_segs, mean_ld;   // mean_ld = n_tiles * BN
 };
 
 // clock64 stamps of CTA 0's pipeline hand-offs: compiled in only in the development build (libfrcnn_b200_wd.so, -DFRCNN_WATCHDOG).
@@ -99,7 +106,10 @@ template <int BN, int MODE> constexpr int stage_bytes() { return KTraits<MODE>::
 template <int BN, int MODE> constexpr int smem_bytes() {
   return STAGES * stage_bytes<BN, MODE>() + 1024 /*align slack*/ + 64 /*barriers*/;
 }
-static_assert(smem_bytes<128, FRCNN_CONV_F16X3>() <= 227 * 1024, "ring exceeds the sm_90 shared-memory limit per block");
+// mean epilogue: one 64-column slice of the 128-row tile at a time, rows padded against bank conflicts
+constexpr int MEAN_COLS = 64, MEAN_LD = MEAN_COLS + 2;
+constexpr int MEAN_SMEM = BLOCK_M * MEAN_LD * 4;
+static_assert(smem_bytes<128, FRCNN_CONV_F16X3>() + MEAN_SMEM <= 227 * 1024, "ring exceeds the sm_90 shared-memory limit per block");
 
 // Work unit u (persistent loop: u = blockIdx.x, += gridDim.x) -> output tile + split-K range.
 struct Unit {
@@ -228,8 +238,78 @@ __device__ __forceinline__ int tile_pixel(const ConvKernelParams& p, const Unit&
   return valid ? (int)(((long long)n * p.ho + h) * p.wo + w) : -1;
 }
 
+__device__ __forceinline__ void consumer_bar() { asm volatile("bar.sync 1, %0;" :: "n"(NUM_CONSUMERS) : "memory"); }
+
+// Mean epilogue (flattened pointwise layer: tile row r is pixel w0 + r; cout % 4 == 0).  Per 64-column slice: both
+// warpgroups put their activated values into `buf` (the arithmetic of finish2; a slice's loads are all issued together, as
+// in epilogue_vec), then thread (slot, col) sums the rows of groups slot, slot + 4, ... of the tile and stores the tile
+// partial.  Four interleaved partial sums per group keep the shared-memory loads in flight; the order is fixed
+// (deterministic, no atomics) and a group of hw values still takes at most hw - 1 rounded adds over the tiles it spans.
 template <int BN>
-__device__ __forceinline__ void epilogue_tile(const ConvKernelParams& p, const Unit& t, const float (&acc)[BN / 2], int r0, int q4) {
+__device__ __forceinline__ void epilogue_mean(const ConvKernelParams& p, const Unit& t, const float (&acc)[BN / 2], int r0, int q4,
+                                              float* buf) {
+  constexpr int CH = MEAN_COLS / 8;
+  const int nrows = min(p.tw, p.wo - t.w0);
+  const int hw = p.mean_hw;
+  const int g0 = t.w0 / hw, nseg = (t.w0 + nrows - 1) / hw - g0 + 1;
+  const int mt = t.w0 / p.tw;
+  const size_t ld = (size_t)p.mean_ld;
+  const int tid = threadIdx.x, col = tid % MEAN_COLS;
+  const bool v0 = r0 < nrows, v1 = r0 + 8 < nrows;
+  const float* const res0 = p.residual ? p.residual + (size_t)(t.w0 + (v0 ? r0 : 0)) * p.cout : nullptr;
+  const float* const res1 = p.residual ? p.residual + (size_t)(t.w0 + (v1 ? r0 + 8 : 0)) * p.cout : nullptr;
+#pragma unroll
+  for (int cc = 0; cc < BN; cc += MEAN_COLS) {
+    float2 sc[CH], sh[CH], ra[CH], rb[CH];
+#pragma unroll
+    for (int jj = 0; jj < CH; ++jj) {
+      const int c = t.nblk * BN + cc + 8 * jj + 2 * q4;
+      sc[jj] = ld_nc_f2_pinned(p.scale + c);          // padded to the tile grid
+      sh[jj] = ld_nc_f2_pinned(p.shift + c);
+      ra[jj] = ld_nc_f2_pinned_if(res0 + c, res0 && v0 && c < p.cout);
+      rb[jj] = ld_nc_f2_pinned_if(res1 + c, res1 && v1 && c < p.cout);
+    }
+    consumer_bar();                                     // the previous slice's sums have read buf
+#pragma unroll
+    for (int jj = 0; jj < CH; ++jj) {
+      const int j = cc / 8 + jj;
+      float2 y0 = make_float2(__fadd_rn(__fmul_rn(acc[4 * j], sc[jj].x), sh[jj].x), __fadd_rn(__fmul_rn(acc[4 * j + 1], sc[jj].y), sh[jj].y));
+      float2 y1 = make_float2(__fadd_rn(__fmul_rn(acc[4 * j + 2], sc[jj].x), sh[jj].x), __fadd_rn(__fmul_rn(acc[4 * j + 3], sc[jj].y), sh[jj].y));
+      if (p.residual) {
+        y0.x = __fadd_rn(y0.x, ra[jj].x); y0.y = __fadd_rn(y0.y, ra[jj].y);
+        y1.x = __fadd_rn(y1.x, rb[jj].x); y1.y = __fadd_rn(y1.y, rb[jj].y);
+      }
+      if (p.act != FRCNN_ACT_NONE) {
+        y0.x = fmaxf(y0.x, 0.f); y0.y = fmaxf(y0.y, 0.f); y1.x = fmaxf(y1.x, 0.f); y1.y = fmaxf(y1.y, 0.f);
+        if (p.act == FRCNN_ACT_RELU6) { y0.x = fminf(y0.x, 6.f); y0.y = fminf(y0.y, 6.f); y1.x = fminf(y1.x, 6.f); y1.y = fminf(y1.y, 6.f); }
+      }
+      *reinterpret_cast<float2*>(buf + r0 * MEAN_LD + 8 * jj + 2 * q4) = y0;
+      *reinterpret_cast<float2*>(buf + (r0 + 8) * MEAN_LD + 8 * jj + 2 * q4) = y1;
+    }
+    consumer_bar();
+    for (int s = tid / MEAN_COLS; s < nseg; s += NUM_CONSUMERS / MEAN_COLS) {
+      const int g = g0 + s;
+      const int rs = max(g * hw - t.w0, 0), re = min((g + 1) * hw - t.w0, nrows);
+      const float* b = buf + col;
+      float a0 = b[rs * MEAN_LD], a1 = 0.f, a2 = 0.f, a3 = 0.f;
+      int r = rs + 1;
+      for (; r + 3 < re; r += 4) {
+        a1 = __fadd_rn(a1, b[r * MEAN_LD]); a2 = __fadd_rn(a2, b[(r + 1) * MEAN_LD]);
+        a3 = __fadd_rn(a3, b[(r + 2) * MEAN_LD]); a0 = __fadd_rn(a0, b[(r + 3) * MEAN_LD]);
+      }
+      for (; r < re; ++r) a1 = __fadd_rn(a1, b[r * MEAN_LD]);
+      p.mean_ws[((size_t)mt * p.mean_segs + s) * ld + (size_t)t.nblk * BN + cc + col] = __fadd_rn(__fadd_rn(a0, a1), __fadd_rn(a2, a3));
+    }
+  }
+}
+
+template <int BN>
+__device__ __forceinline__ void epilogue_tile(const ConvKernelParams& p, const Unit& t, const float (&acc)[BN / 2], int r0, int q4,
+                                              float* mean_buf) {
+  if (p.mean_out) {                                     // mean layers are never split (decide_geometry)
+    epilogue_mean<BN>(p, t, acc, r0, q4, mean_buf);
+    return;
+  }
   if (t.slot >= 0) {
     // split tile: raw partial sums into the tile-local [128][BN] workspace (row-major); tail_reduce_kernel runs the epilogue
     float* const w = p.ws + ((size_t)t.slot * p.splits + t.z) * (size_t)(BLOCK_M * BN) + 2 * q4;
@@ -259,8 +339,8 @@ __device__ __forceinline__ void wgmma_rs(float (&d)[BN / 2], const uint32_t (&a)
 
 template <int BN, int MODE>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmBhi,
-                 const __grid_constant__ CUtensorMap tmBlo, const ConvKernelParams p) {
+conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
+                 const __grid_constant__ CUtensorMap tmBhi, const __grid_constant__ CUtensorMap tmBlo, const ConvKernelParams p) {
   using T = KTraits<MODE>;
   constexpr int kStage = stage_bytes<BN, MODE>();
   constexpr int kPlane = b_plane_bytes<BN>();
@@ -272,6 +352,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   // stage s: [A box 0 (| A box 1)] [B hi] [B lo], every part 1024-B aligned (SWIZZLE_128B atoms)
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * kStage);   // A and B bytes of the stage landed (tx)
   uint64_t* empty = full + STAGES;                                        // both warpgroups are done with the stage
+  // full + 8 (64 B of barriers on): MEAN_SMEM bytes for the mean epilogue, allocated only when it is on
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -279,6 +360,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
   if (threadIdx.x == NUM_CONSUMERS) {
     tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmBhi); tma_prefetch_desc(&tmBlo);
+    if (p.cin2) tma_prefetch_desc(&tmA2);
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], NUM_CONSUMERS); }
     mbar_fence_init();
   }
@@ -293,7 +375,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     reg_dec<REGS_PRODUCER>();
     if (warp == NUM_CONSUMERS / 32 && lane == 0) {
       const int cchunks = p.cin / BLOCK_K;                        // 32-channel chunks per filter tap
-      const int total32 = p.kh * p.kw * cchunks;
+      const int total1 = p.kh * p.kw * cchunks;                   // ... of the first source; then cin2 / 32 of the second
+      const int cchunks2 = p.cin2 / BLOCK_K;
       const uint32_t tx = (uint32_t)(T::BOXES * p.a_box_bytes + (T::X1 ? 1 : 2) * kPlane);
       int s = 0; uint32_t ph = 0, kbt = 0;
       for (int u = blockIdx.x; u < p.total_units; u += gridDim.x) {
@@ -307,9 +390,14 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           for (int i = 0; i < T::BOXES; ++i) {
             const int g32 = (t.kb0 + kb) * T::BOXES + i;           // global 32-channel block -> (filter tap, channel chunk)
             int tap = g32 / cchunks, kc = g32 - tap * cchunks;
-            if (g32 >= total32) { tap = 0; kc = cchunks; }        // odd tail: a box past the last channel is zero-filled by TMA
+            const CUtensorMap* ma = &tmA;
+            if (g32 >= total1) {                                  // second source (pointwise: one tap), or the odd tail: a box
+              tap = 0;                                            // past the last channel is zero-filled by TMA
+              if (cchunks2) { ma = &tmA2; kc = min(g32 - total1, cchunks2); }
+              else kc = cchunks;
+            }
             const int r = tap / p.kw, sx = tap - r * p.kw;
-            tma_load_4d(st + i * A_TILE_BYTES, &tmA, &full[s], kc * BLOCK_K, t.w0 * p.stride + sx - p.pad_l,
+            tma_load_4d(st + i * A_TILE_BYTES, ma, &full[s], kc * BLOCK_K, t.w0 * p.stride + sx - p.pad_l,
                         t.h0 * p.stride + r - p.pad_t, t.n0);
           }
           const int kcoord = (t.kb0 + kb) * T::BOXES * BLOCK_K;   // K axis of the packed weights = (tap, cin) flattened; past the end: zeros
@@ -407,7 +495,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       if (threadIdx.x == 0) FRCNN_TRACE(2, kbt);
       if (++s == STAGES) { s = 0; ph ^= 1u; }
     }
-    epilogue_tile<BN>(p, t, acc, r0, q4);
+    epilogue_tile<BN>(p, t, acc, r0, q4, reinterpret_cast<float*>(full + 8));
   }
 }
 
@@ -466,6 +554,29 @@ tail_reduce_kernel(const ConvKernelParams p) {
   }
 }
 
+// Second pass of the mean epilogue: mean_out[g][c] = (tile partials of group g, added in tile order) / mean_hw.  A group's
+// pixels lie in one or two tiles when mean_hw <= tile width (more for longer groups); thread = (group, channel).
+__global__ void __launch_bounds__(256)
+mean_finish_kernel(const ConvKernelParams p) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const long gid = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int groups = p.wo / p.mean_hw;
+  if (gid >= (long)groups * p.cout) return;
+  const int c = (int)(gid % p.cout), g = (int)(gid / p.cout);
+  const int hw = p.mean_hw;
+  const size_t ld = (size_t)p.mean_ld;
+  const long p0 = (long)g * hw, p1 = p0 + hw - 1;
+  const int m0 = (int)(p0 / p.tw), m1 = (int)(p1 / p.tw);
+  float sum = 0.f;
+  for (int m = m0; m <= m1; ++m) {
+    const int s = g - (int)(((long)m * p.tw) / hw);
+    const float v = p.mean_ws[((size_t)m * p.mean_segs + s) * ld + c];
+    sum = m == m0 ? v : __fadd_rn(sum, v);
+  }
+  p.mean_out[(size_t)g * p.cout + c] = __fdiv_rn(sum, (float)hw);
+}
+
 // plan creation: the epilogue's per-channel vectors, padded to the tile grid (no bounds tests in the kernel)
 __global__ void prep_epilogue_vectors_kernel(const float* scale, const float* shift, float out_mult, int cout, int padded,
                                              float* eff_scale, float* eff_shift) {
@@ -519,7 +630,7 @@ static int encode_map(CUtensorMap* m, const void* base, int rank, const uint64_t
 using namespace frcnn;
 
 struct frcnn_conv_plan {
-  CUtensorMap tmA, tmBhi, tmBlo;
+  CUtensorMap tmA, tmA2, tmBhi, tmBlo;   // tmA2: the second A source, or a copy of tmA
   ConvKernelParams kp;
   int block_n, stages, smem;
   int impl;                // FRCNN_CONV_F16X3 | FRCNN_CONV_TF32X3 | FRCNN_CONV_F16X1
@@ -527,6 +638,7 @@ struct frcnn_conv_plan {
   int n_tail;
   float* ws;               // owned workspace of the split tiles 
   float* eff;              // owned epilogue vectors: scale * out_mult | shift, each padded to n_tiles * block_n
+  float* mean_ws;          // owned tile partials of the mean epilogue
 };
 
 // choose the tile of output pixels (tn x th x tw <= 128) that needs the fewest tiles
@@ -562,7 +674,8 @@ template <int BN, int MODE>
 static int launch(const frcnn_conv_plan* p, cudaStream_t st) {
   static bool attr_done = false;
   if (!attr_done) {
-    FRCNN_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes<BN, MODE>()));
+    FRCNN_CUDA(cudaFuncSetAttribute(conv_gemm_kernel<BN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    smem_bytes<BN, MODE>() + MEAN_SMEM));
     attr_done = true;
   }
   cudaLaunchAttribute attr[1];
@@ -570,9 +683,17 @@ static int launch(const frcnn_conv_plan* p, cudaStream_t st) {
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   const bool pdl = pdl_enabled();
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = p->grid; cfg.blockDim = dim3(NUM_THREADS); cfg.dynamicSmemBytes = smem_bytes<BN, MODE>(); cfg.stream = st;
+  cfg.gridDim = p->grid; cfg.blockDim = dim3(NUM_THREADS); cfg.stream = st;
+  cfg.dynamicSmemBytes = smem_bytes<BN, MODE>() + (p->kp.mean_out ? MEAN_SMEM : 0);
   cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-  FRCNN_CUDA(cudaLaunchKernelEx(&cfg, conv_gemm_kernel<BN, MODE>, p->tmA, p->tmBhi, p->tmBlo, p->kp));
+  FRCNN_CUDA(cudaLaunchKernelEx(&cfg, conv_gemm_kernel<BN, MODE>, p->tmA, p->tmA2, p->tmBhi, p->tmBlo, p->kp));
+  if (p->kp.mean_out) {
+    cudaLaunchConfig_t mc{};
+    const long n = (long)(p->kp.wo / p->kp.mean_hw) * p->kp.cout;
+    mc.gridDim = dim3((unsigned)((n + 255) / 256)); mc.blockDim = dim3(256); mc.dynamicSmemBytes = 0; mc.stream = st;
+    mc.attrs = attr; mc.numAttrs = pdl ? 1 : 0;
+    FRCNN_CUDA(cudaLaunchKernelEx(&mc, mean_finish_kernel, p->kp));
+  }
   if (p->n_tail > 0) {
     cudaLaunchConfig_t rc{};
     rc.gridDim = dim3((unsigned)(p->n_tail * (BLOCK_M / (256 / (BN / 4))))); rc.blockDim = dim3(256); rc.dynamicSmemBytes = 0; rc.stream = st;
@@ -602,15 +723,24 @@ static int decide_geometry(const frcnn_conv_desc* d, int sms, Geometry* g) {
   FRCNN_REQUIRE(sms > 0, "bad SM count");
   g->n = d->n; g->h = d->h; g->w = d->w; g->ho = d->ho; g->wo = d->wo;
   const bool pointwise = d->kh == 1 && d->kw == 1 && d->stride == 1 && d->pad_t == 0 && d->pad_l == 0 && g->ho == g->h && g->wo == g->w;
+  const bool mean = d->mean_hw != 0;
+  FRCNN_REQUIRE(d->cin2 >= 0 && d->cin2 % BLOCK_K == 0, "cin2=%d must be 0 or a positive multiple of 32", d->cin2);
+  FRCNN_REQUIRE(d->cin2 == 0 || pointwise, "a second A source needs a pointwise layer (1x1, stride 1, no padding)");
+  FRCNN_REQUIRE(!mean || pointwise, "the mean epilogue needs a pointwise layer (1x1, stride 1, no padding)");
+  FRCNN_REQUIRE(!mean || d->cout % 4 == 0, "the mean epilogue needs cout %% 4 == 0 (cout=%d)", d->cout);
+  FRCNN_REQUIRE(d->mean_hw >= 0 && (!mean || ((long)d->n * d->h * d->w) % d->mean_hw == 0),
+                "mean_hw=%d must be positive and divide the pixel count", d->mean_hw);
+  FRCNN_REQUIRE(!mean || d->split_k <= 1, "the mean epilogue is never split along K");
   if (pointwise) {  // flatten all pixels into one row of "width" n*h*w: perfect 128-row tiles
     g->w = g->wo = g->n * g->h * g->w; g->n = 1; g->h = g->ho = 1;
   }
+  const int ktot = d->kh * d->kw * d->cin + d->cin2;             // K of the packed weights
   choose_tile(g->n, g->ho, g->wo, d->stride, &g->tn, &g->th, &g->tw);
   g->tiles_w = cdiv(g->wo, g->tw); g->tiles_h = cdiv(g->ho, g->th); g->tiles_n = cdiv(g->n, g->tn);
   g->m_tiles = (long)g->tiles_w * g->tiles_h * g->tiles_n;
   const bool f16 = d->impl != FRCNN_CONV_TF32X3;
   const int ks = f16 ? 2 : 1;                                   // 32-channel blocks per k-block (f16x3: 64-wide k-blocks)
-  g->num_kb = cdiv(d->kh * d->kw * d->cin / BLOCK_K, ks);
+  g->num_kb = cdiv(ktot / BLOCK_K, ks);
   g->kpc = d->kb_per_chunk > 0 ? d->kb_per_chunk : 8 / ks;
   int bn = d->block_n;
   if (bn == 0) {
@@ -649,7 +779,8 @@ static int decide_geometry(const frcnn_conv_desc* d, int sms, Geometry* g) {
   }
   int kbs = cdiv(num_kb, splits);                              // (a unit's last chunk may be shorter than kb_per_chunk)
   splits = cdiv(num_kb, kbs);
-  if (splits < 2 || (d->cout & 3) != 0) { n_tail = 0; splits = 1; kbs = num_kb; }   // tail_reduce_kernel reads the padded epilogue vectors as float4
+  // tail_reduce_kernel reads the padded epilogue vectors as float4; the mean epilogue sums whole tiles
+  if (splits < 2 || (d->cout & 3) != 0 || mean) { n_tail = 0; splits = 1; kbs = num_kb; }
   FRCNN_REQUIRE(splits <= 64, "bad split_k");
   g->n_tail = n_tail; g->splits = splits; g->kbs = kbs;
   g->total_units = (g->tiles - n_tail) + n_tail * splits;
@@ -657,7 +788,7 @@ static int decide_geometry(const frcnn_conv_desc* d, int sms, Geometry* g) {
   g->grid = (int)(g->total_units < sms ? g->total_units : sms);   // persistent: one CTA per SM walks the units
   {
     const char* e = getenv("FRCNN_CONV_RASTER");          // development override: m | n
-    const double a_bytes = (double)d->n * d->h * d->w * d->cin * 4.0, b_bytes = (double)d->cout * d->kh * d->kw * d->cin * 4.0;
+    const double a_bytes = (double)d->n * d->h * d->w * (d->cin + d->cin2) * 4.0, b_bytes = (double)d->cout * ktot * 4.0;
     g->raster_n = (e && (e[0] == 'm' || e[0] == 'n')) ? (e[0] == 'n') : (a_bytes > b_bytes && g->n_tiles > 1);
   }
   return OK;
@@ -676,7 +807,9 @@ extern "C" int frcnn_conv_plan_geometry(const frcnn_conv_desc* d, int sm_count, 
 
 extern "C" int frcnn_conv_plan_create(frcnn_conv_plan** out, const frcnn_conv_desc* d) {
   FRCNN_REQUIRE(out && d, "null argument");
-  FRCNN_REQUIRE(d->in_dev && d->w_hi_dev && d->w_lo_dev && d->out_dev, "null device pointer");
+  FRCNN_REQUIRE(d->in_dev && d->w_hi_dev && d->w_lo_dev && (d->mean_hw ? d->mean_dev != nullptr : d->out_dev != nullptr),
+                "null device pointer");
+  FRCNN_REQUIRE(d->cin2 == 0 || d->in2_dev, "cin2=%d without in2_dev", d->cin2);
   int sms = 132;
   { int dev = 0; cudaDeviceProp pr; if (cudaGetDevice(&dev) == cudaSuccess && cudaGetDeviceProperties(&pr, dev) == cudaSuccess && pr.multiProcessorCount > 0) sms = pr.multiProcessorCount; }
   Geometry g;
@@ -694,10 +827,17 @@ extern "C" int frcnn_conv_plan_create(frcnn_conv_plan** out, const frcnn_conv_de
     uint32_t es[4] = {1, (uint32_t)d->stride, (uint32_t)d->stride, 1};
     int rc = encode_map(&p->tmA, d->in_dev, 4, dims, strides, box, es);
     if (rc) { free(p); return rc; }
+    p->tmA2 = p->tmA;
+    if (d->cin2 > 0) {   // pointwise: same pixel rows, cin2 channels
+      uint64_t dims2[4] = {(uint64_t)d->cin2, (uint64_t)g.w, (uint64_t)g.h, (uint64_t)g.n};
+      uint64_t strides2[3] = {(uint64_t)d->cin2 * 4, (uint64_t)g.w * d->cin2 * 4, (uint64_t)g.h * g.w * d->cin2 * 4};
+      rc = encode_map(&p->tmA2, d->in2_dev, 4, dims2, strides2, box, es);
+      if (rc) { free(p); return rc; }
+    }
   }
   const bool f16 = d->impl != FRCNN_CONV_TF32X3;
   {
-    const uint64_t ktot = (uint64_t)d->kh * d->kw * d->cin;
+    const uint64_t ktot = (uint64_t)d->kh * d->kw * d->cin + d->cin2;
     uint64_t dims[2] = {ktot, (uint64_t)d->cout};
     uint64_t strides[1] = {ktot * (f16 ? 2 : 4)};
     uint32_t box[2] = {(uint32_t)(f16 ? 2 * BLOCK_K : BLOCK_K), (uint32_t)bn};   // 128-byte rows either way
@@ -721,7 +861,10 @@ extern "C" int frcnn_conv_plan_create(frcnn_conv_plan** out, const frcnn_conv_de
   k.kb_per_split = g.kbs; k.splits = g.splits; k.n_full = (int)(g.tiles - g.n_tail);
   k.total_units = (int)g.total_units;
   k.raster_n = g.raster_n;
-  k.ws = nullptr; p->ws = nullptr; p->eff = nullptr; p->n_tail = (int)g.n_tail;
+  k.cin2 = d->cin2;
+  k.mean_out = d->mean_hw ? d->mean_dev : nullptr; k.mean_ws = nullptr; k.mean_hw = d->mean_hw; k.mean_ld = g.n_tiles * bn;
+  k.mean_segs = d->mean_hw ? (g.tw < cdiv(g.tw - 1, d->mean_hw) + 1 ? g.tw : cdiv(g.tw - 1, d->mean_hw) + 1) : 0;
+  k.ws = nullptr; p->ws = nullptr; p->eff = nullptr; p->mean_ws = nullptr; p->n_tail = (int)g.n_tail;
   {
     // NOTE: the vectors are snapshots of scale_dev / shift_dev taken now (they are weights: constant after load)
     const int padded = g.n_tiles * bn;
@@ -739,12 +882,18 @@ extern "C" int frcnn_conv_plan_create(frcnn_conv_plan** out, const frcnn_conv_de
     if (e != cudaSuccess) { cudaFree(p->eff); free(p); return cuda_fail(e, "split-tile workspace", __FILE__, __LINE__); }
     k.ws = p->ws;
   }
+  if (d->mean_hw) {
+    cudaError_t e = cudaMalloc(&p->mean_ws, (size_t)g.m_tiles * k.mean_segs * k.mean_ld * sizeof(float));
+    if (e != cudaSuccess) { cudaFree(p->eff); free(p); return cuda_fail(e, "mean workspace", __FILE__, __LINE__); }
+    k.mean_ws = p->mean_ws;
+  }
   p->grid = dim3((unsigned)g.grid, 1, 1);
   p->block_n = bn;
   p->impl = f16 ? (d->impl == FRCNN_CONV_F16X1 ? FRCNN_CONV_F16X1 : FRCNN_CONV_F16X3) : FRCNN_CONV_TF32X3;
   p->stages = STAGES;
   p->smem = f16 ? (bn == 128 ? smem_bytes<128, FRCNN_CONV_F16X3>() : smem_bytes<64, FRCNN_CONV_F16X3>())
               : (bn == 128 ? smem_bytes<128, FRCNN_CONV_TF32X3>() : smem_bytes<64, FRCNN_CONV_TF32X3>());
+  if (d->mean_hw) p->smem += MEAN_SMEM;
   *out = p;
   return OK;
 }
@@ -794,5 +943,6 @@ extern "C" int frcnn_conv_plan_set_trace(frcnn_conv_plan* p, long long* trace_de
 extern "C" void frcnn_conv_plan_destroy(frcnn_conv_plan* p) {
   if (p && p->ws) cudaFree(p->ws);
   if (p && p->eff) cudaFree(p->eff);
+  if (p && p->mean_ws) cudaFree(p->mean_ws);
   free(p);
 }

@@ -29,6 +29,17 @@ def bn_fold(gamma, beta, mean, var, eps):
     return inv, (beta.astype(F) - mean.astype(F) * inv).astype(F)
 
 
+def concat_layers(weights, names, bn_eps):
+    """(w, scale, shift) of Weights.packed_concat on the host: w = [W_1 diag(s_1) ; ...] fp32, scale None, shift = the shifts
+    added in order in fp32."""
+    ss = [weights.scale_shift(nm, bn_eps) for nm in names]
+    w = ops.concat_scaled_weights([weights[nm + "/weights"] for nm in names], [s for s, _ in ss])
+    shift = ss[0][1]
+    for _, sh in ss[1:]:
+        shift = (shift + sh).astype(F)
+    return w, None, shift
+
+
 class Weights:
     """TF-variable-name -> numpy store plus a cache of device-packed layers (packed once per network)."""
 
@@ -61,6 +72,15 @@ class Weights:
             sc, sh = self.scale_shift(name, bn_eps)
             self._packed[name] = ops.PackedConv(self.t[name + w_key], sc, sh)
         return self._packed[name]
+
+    def packed_concat(self, names, bn_eps):
+        """One 1x1 layer computing the sum of the BatchNorm'd 1x1 layers `names` over their concatenated inputs:
+        weights [W_1 diag(s_1) ; W_2 diag(s_2) ; ...] (scales folded in fp32, one weight exponent for the whole matrix),
+        epilogue scale 1 and shift = the sum of the shifts in fp32."""
+        key = "+".join(names)
+        if key not in self._packed:
+            self._packed[key] = ops.PackedConv(*concat_layers(self, names, bn_eps))
+        return self._packed[key]
 
     def packed_custom(self, key, build):
         """build() -> (w_hwio, scale, shift) for fused layers (RPN heads, cls+bbox)."""
@@ -133,12 +153,14 @@ class Tape:
             fn()
 
     # ---- dense layers -------------------------------------------------------------------------------
-    def conv(self, x, name, stride=1, mode="SAME", act=N.ACT_RELU, bn_eps=None, residual=None, packed=None):
+    def conv(self, x, name, stride=1, mode="SAME", act=N.ACT_RELU, bn_eps=None, residual=None, packed=None, x2=None, mean=False):
+        """x2: second input of a pointwise layer whose packed weights cover both inputs' channels (Weights.packed_concat).
+        mean: return [n, cout], each image's spatial mean of the activated output (the output map is never stored)."""
         pc = packed if packed is not None else self.w.packed_conv(name, bn_eps)
         n, h, w, _ = x.shape
         ho, wo, pt, pl = ops.conv_out_hw(h, w, pc.kh, stride, mode)
-        out = self.new(n, ho, wo, pc.cout)
-        plan = ops.ConvPlan(x, pc, out, stride, pt, pl, act, residual)
+        out = self.new(n, pc.cout) if mean else self.new(n, ho, wo, pc.cout)
+        plan = ops.ConvPlan(x, pc, out, stride, pt, pl, act, residual, x2=x2, mean=mean)
         self.conv_plans.append(plan)
         self.add("conv:" + name, plan.run)
         fl = 2.0 * n * ho * wo * pc.cout * pc.kh * pc.kw * pc.cin

@@ -82,21 +82,45 @@ class PackedConv:
         self.shift = None if shift is None else torch.as_tensor(np.ascontiguousarray(shift), dtype=torch.float32).cuda()
 
 
-class ConvPlan:
-    """frcnn_conv_plan bound to fixed input/output/residual buffers (TMA descriptors hold raw pointers)."""
+def concat_scaled_weights(ws, scales):
+    """[W_1 diag(s_1) ; W_2 diag(s_2) ; ...] for 1x1 layers summed into one output: HWIO [1, 1, cin_i, cout] weights, each
+    times its per-output-channel scale (None = 1) in fp32, stacked along cin -> HWIO [1, 1, sum cin_i, cout] fp32."""
+    parts = []
+    for w, s in zip(ws, scales):
+        w = np.asarray(w, dtype=np.float32)
+        assert w.ndim == 4 and w.shape[:2] == (1, 1), w.shape
+        parts.append(w if s is None else (w * np.asarray(s, dtype=np.float32)).astype(np.float32))
+    return np.ascontiguousarray(np.concatenate(parts, axis=2))
 
-    def __init__(self, x, pc, out, stride=1, pad_t=0, pad_l=0, act=N.ACT_NONE, residual=None, block_n=0, kb_per_chunk=0, split_k=0):
+
+class ConvPlan:
+    """frcnn_conv_plan bound to fixed input/output/residual buffers (TMA descriptors hold raw pointers).
+
+    x2: second A source of a pointwise layer (pc packs [cin + cin2] input channels; x2 holds the last cin2).
+    mean: out is [n, cout], the mean over each image's h*w activated outputs (pointwise layers), computed in the epilogue."""
+
+    def __init__(self, x, pc, out, stride=1, pad_t=0, pad_l=0, act=N.ACT_NONE, residual=None, block_n=0, kb_per_chunk=0, split_k=0,
+                 x2=None, mean=False):
         _f32(x); _f32(out)
         n, h, w, cin = x.shape
-        assert cin == pc.cin, (cin, pc.cin)
-        no, ho, wo, co = out.shape
-        assert no == n and co == pc.cout
-        d = N.ConvDesc(_p(x), _p(pc.w_hi), _p(pc.w_lo), _p(pc.scale), _p(pc.shift), _p(residual), _p(out),
+        cin2 = 0
+        if x2 is not None:
+            _f32(x2)
+            assert x2.shape[:3] == x.shape[:3], (x2.shape, x.shape)
+            cin2 = int(x2.shape[3])
+        assert cin + cin2 == pc.cin, (cin, cin2, pc.cin)
+        if mean:
+            ho, wo = h, w
+            assert tuple(out.shape) == (n, pc.cout), (out.shape, n, pc.cout)
+        else:
+            no, ho, wo, co = out.shape
+            assert no == n and co == pc.cout
+        d = N.ConvDesc(_p(x), _p(pc.w_hi), _p(pc.w_lo), _p(pc.scale), _p(pc.shift), _p(residual), _p(None if mean else out),
                        n, h, w, cin, pc.cout, pc.kh, pc.kw, stride, pad_t, pad_l, ho, wo, act, block_n, kb_per_chunk, split_k,
-                       pc.impl, pc.out_mult)
+                       pc.impl, pc.out_mult, _p(x2), cin2, _p(out if mean else None), h * w if mean else 0)
         self._h = C.c_void_p()
         N.check(N.lib().frcnn_conv_plan_create(C.byref(self._h), C.byref(d)), "conv_plan_create")
-        self._keep = (x, pc, out, residual)
+        self._keep = (x, pc, out, residual, x2)
         self.flops = 2.0 * n * ho * wo * pc.cout * pc.kh * pc.kw * pc.cin
 
     def run(self):
