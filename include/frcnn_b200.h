@@ -213,6 +213,19 @@ int frcnn_proposals(const float* props_dev, const float* scores_dev, const int* 
  * pre_pool 0: direct 7x7, 1: 14x14 then 2x2/2 max.  out [r,7,7,c] */
 int frcnn_crop_pool(const float* feat_dev, int batch, int fh, int fw, int c, const float* rois_dev, int r, int pooled,
                     int pre_pool, float* out_dev, void* stream);
+/* POOLING_MODE 'align' (extension): torchvision.ops.roi_align(spatial_scale, sampling_ratio, aligned) on NHWC, each fp32
+ * operation rounded once (no contraction); a sample outside [-1, dim] is not read.  feat_dev [batch,fh,fw,c], c % 4 == 0;
+ * rois_dev [r,5] = (image index clamped to [0, batch-1], x1, y1, x2, y2 in blob pixels); 1 <= pooled <= 16;
+ * 0 <= sampling_ratio <= FRCNN_ROI_ALIGN_MAX_SAMPLING (0 = adaptive, ceil(roi size / pooled) per axis: the launch walks every
+ * sample, so the caller keeps boxes bounded -- RPN RoIs lie inside the blob, caller boxes within [-W,2W] x [-H,2H]).
+ * out_dev [r,pooled,pooled,c]. */
+#define FRCNN_ROI_ALIGN_MAX_SAMPLING 16
+int frcnn_roi_align(const float* feat_dev, int batch, int fh, int fw, int c, const float* rois_dev, int r, int pooled,
+                    float spatial_scale, int sampling_ratio, int aligned, float* out_dev, void* stream);
+/* POOLING_MODE 'pool' (extension): torchvision.ops.roi_pool -- corners round(x*spatial_scale) half away from zero, bins of
+ * max(size+1,1)/pooled cells, max by '>' from -FLT_MAX (empty bin: 0).  Arguments as frcnn_roi_align. */
+int frcnn_roi_pool(const float* feat_dev, int batch, int fh, int fw, int c, const float* rois_dev, int r, int pooled,
+                   float spatial_scale, float* out_dev, void* stream);
 /* split the fused [r, ld] head GEMM output (cls logits at col 0, 4C deltas at col C):
  * cls_score [r,C], cls_prob = softmax, bbox_pred = delta*stds + means (network.py:361-378,428-432) */
 int frcnn_cls_finish(const float* head_out_dev, int ld, int r, int num_classes, const float* stds4,

@@ -19,6 +19,8 @@ CONV_F16X3, CONV_TF32X3, CONV_F16X1 = 0, 1, 2
 SOFT_NMS_METHODS = {"linear": 0, "gaussian": 1, "hard": 2}   # FRCNN_SOFT_NMS_*
 AUG_MAX_VIEWS = 16                                            # FRCNN_AUG_MAX_VIEWS
 BOX_VOTE_METHODS = {"ID": 0, "AVG": 1, "IOU_AVG": 2, "GENERALIZED_AVG": 3, "QUASI_SUM": 4, "TEMP_AVG": 5}   # FRCNN_BOX_VOTE_*
+ROI_ALIGN_MAX_SAMPLING = 16                                   # FRCNN_ROI_ALIGN_MAX_SAMPLING
+ROI_MAX_POOLED = 16                                           # pooled sizes 1..16 of frcnn_roi_align / frcnn_roi_pool
 
 vp, ci, cf, cu, sz = C.c_void_p, C.c_int, C.c_float, C.c_uint, C.c_size_t
 ip, fp = C.POINTER(C.c_int), C.POINTER(C.c_float)
@@ -64,6 +66,8 @@ SIGNATURES = {
     "frcnn_sort_desc": (ci, [vp, ci, ci, vp, vp, vp, sz, vp]),
     "frcnn_proposals": (ci, [vp, vp, vp, ci, ci, ci, ci, cf, cu, vp, vp, vp, vp, vp]),
     "frcnn_crop_pool": (ci, [vp, ci, ci, ci, ci, vp, ci, ci, ci, vp, vp]),
+    "frcnn_roi_align": (ci, [vp, ci, ci, ci, ci, vp, ci, ci, cf, ci, ci, vp, vp]),
+    "frcnn_roi_pool": (ci, [vp, ci, ci, ci, ci, vp, ci, ci, cf, vp, vp]),
     "frcnn_cls_finish": (ci, [vp, ci, ci, ci, fp, fp, vp, vp, vp, vp]),
     "frcnn_bbox_decode": (ci, [vp, vp, ci, ci, ci, vp, vp, vp]),
     "frcnn_detect_post_workspace_bytes": (sz, [ci, ci, ci]),

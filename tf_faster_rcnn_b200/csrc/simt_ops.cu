@@ -298,6 +298,146 @@ crop_pool_kernel(const float* __restrict__ feat, int batch, int fh, int fw, int 
   }
 }
 
+// ---- RoIAlign / RoIPool (POOLING_MODE 'align' / 'pool') ------------------------------------------------------
+// torchvision.ops.roi_align / roi_pool on NHWC, op by op in fp32 (DESIGN §2 gives the definition the tests pin).
+// One block per (RoI, output row) as crop_pool_kernel.
+constexpr int ROI_MAX_POOLED = 16;
+constexpr int ALIGN_XTAB = 512;     // x-sample entries per pass, (pw, ix) pairs
+constexpr int ALIGN_YTAB = 64;      // y-sample entries per pass
+
+// One sample coordinate of one axis: neighbour offsets (row offsets premultiplied by fw), their weights; lo < 0 = the sample
+// lies outside [-1, dim] and contributes nothing.
+struct __align__(16) AxisSample { int lo, hi; float l, h; };
+
+__device__ __forceinline__ AxisSample align_axis(float v, int dim, int mult) {
+  AxisSample s;
+  if (v < -1.f || v > (float)dim) { s.lo = s.hi = -1; s.l = s.h = 0.f; return s; }
+  if (v <= 0.f) v = 0.f;
+  int lo = (int)v, hi;
+  if (lo >= dim - 1) { lo = hi = dim - 1; v = (float)lo; } else { hi = lo + 1; }
+  s.l = __fsub_rn(v, (float)lo);
+  s.h = __fsub_rn(1.f, s.l);
+  s.lo = lo * mult; s.hi = hi * mult;
+  return s;
+}
+
+__device__ __forceinline__ float align_term(float acc, float w1, float w2, float w3, float w4, float v1, float v2, float v3, float v4) {
+  return __fadd_rn(acc, __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(w1, v1), __fmul_rn(w2, v2)), __fmul_rn(w3, v3)), __fmul_rn(w4, v4)));
+}
+
+// The sample geometry is separable: a y table over (iy) and an x table over (pw, ix), built by the block once per pass; every
+// thread then streams float4 channel groups through the samples in (iy, ix) order.  A grid too large for the tables is walked
+// in passes that keep that order (whole rows of iy while every ix fits, else one iy row and a range of ix per pass), the
+// running sum carried between passes in the output element itself (an fp32 store and reload is exact).
+__global__ void __launch_bounds__(256)
+roi_align_kernel(const float* __restrict__ feat, int batch, int fh, int fw, int c, const float* __restrict__ rois, int pooled,
+                 float scale, int sampling_ratio, int aligned, float* __restrict__ out) {
+  __shared__ AxisSample ytab[ALIGN_YTAB];
+  __shared__ AxisSample xtab[ALIGN_XTAB];
+  const int ri = blockIdx.x / pooled, ph = blockIdx.x % pooled;
+  const float* roi = rois + (size_t)ri * 5;
+  const int bi = min(max((int)__ldg(roi), 0), batch - 1);
+  feat += (size_t)bi * fh * fw * c;
+  const float off = aligned ? 0.5f : 0.f;
+  const float sx = __fsub_rn(__fmul_rn(__ldg(roi + 1), scale), off), sy = __fsub_rn(__fmul_rn(__ldg(roi + 2), scale), off);
+  const float ex = __fsub_rn(__fmul_rn(__ldg(roi + 3), scale), off), ey = __fsub_rn(__fmul_rn(__ldg(roi + 4), scale), off);
+  float rw = __fsub_rn(ex, sx), rh = __fsub_rn(ey, sy);
+  if (!aligned) { rw = rw < 1.f ? 1.f : rw; rh = rh < 1.f ? 1.f : rh; }    // std::max(v, 1): a NaN stays NaN
+  const float bw = __fdiv_rn(rw, (float)pooled), bh = __fdiv_rn(rh, (float)pooled);
+  const int gw = sampling_ratio > 0 ? sampling_ratio : (int)ceilf(bw);
+  const int gh = sampling_ratio > 0 ? sampling_ratio : (int)ceilf(bh);
+  const float cnt = (float)max(gh * gw, 1);
+  const float y0 = __fadd_rn(sy, __fmul_rn((float)ph, bh));
+  const int c4 = c >> 2, items = pooled * c4;
+  float* orow = out + (size_t)blockIdx.x * pooled * c;
+  if (gh <= 0 || gw <= 0) {                       // no sample: 0 / count
+    for (int i = threadIdx.x; i < items; i += blockDim.x) reinterpret_cast<float4*>(orow)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    return;
+  }
+  const int xcap = max(ALIGN_XTAB / pooled, 1);
+  const bool xsplit = gw > xcap;
+  const int ystep = xsplit ? 1 : ALIGN_YTAB, xstep = xsplit ? xcap : gw;
+  for (int iy0 = 0; iy0 < gh; iy0 += ystep) {
+    for (int ix0 = 0; ix0 < gw; ix0 += xstep) {
+      const int ny = min(ystep, gh - iy0), nx = min(xstep, gw - ix0);
+      const bool first = iy0 == 0 && ix0 == 0, last = iy0 + ny == gh && ix0 + nx == gw;
+      __syncthreads();                            // the previous pass's readers are done with the tables
+      for (int k = threadIdx.x; k < ny; k += blockDim.x) {
+        const float y = __fadd_rn(y0, __fdiv_rn(__fmul_rn(__fadd_rn((float)(iy0 + k), 0.5f), bh), (float)gh));
+        ytab[k] = align_axis(y, fh, fw);
+      }
+      for (int k = threadIdx.x; k < pooled * nx; k += blockDim.x) {
+        const int pw = k / nx, ix = ix0 + k - pw * nx;
+        const float x = __fadd_rn(__fadd_rn(sx, __fmul_rn((float)pw, bw)), __fdiv_rn(__fmul_rn(__fadd_rn((float)ix, 0.5f), bw), (float)gw));
+        xtab[k] = align_axis(x, fw, 1);
+      }
+      __syncthreads();
+      for (int i = threadIdx.x; i < items; i += blockDim.x) {
+        const int pw = i / c4, cg = i - pw * c4;
+        float4 acc = first ? make_float4(0.f, 0.f, 0.f, 0.f) : reinterpret_cast<const float4*>(orow)[i];
+        const AxisSample* xs = xtab + pw * nx;
+        for (int iy = 0; iy < ny; ++iy) {
+          const AxisSample ys = ytab[iy];
+          if (ys.lo < 0) continue;
+          const float4* rlo = reinterpret_cast<const float4*>(feat + (size_t)ys.lo * c) + cg;
+          const float4* rhi = reinterpret_cast<const float4*>(feat + (size_t)ys.hi * c) + cg;
+          for (int ix = 0; ix < nx; ++ix) {
+            const AxisSample xv = xs[ix];
+            if (xv.lo < 0) continue;
+            const float w1 = __fmul_rn(ys.h, xv.h), w2 = __fmul_rn(ys.h, xv.l), w3 = __fmul_rn(ys.l, xv.h), w4 = __fmul_rn(ys.l, xv.l);
+            const float4 v1 = __ldg(rlo + (size_t)xv.lo * c4), v2 = __ldg(rlo + (size_t)xv.hi * c4);
+            const float4 v3 = __ldg(rhi + (size_t)xv.lo * c4), v4 = __ldg(rhi + (size_t)xv.hi * c4);
+            acc.x = align_term(acc.x, w1, w2, w3, w4, v1.x, v2.x, v3.x, v4.x);
+            acc.y = align_term(acc.y, w1, w2, w3, w4, v1.y, v2.y, v3.y, v4.y);
+            acc.z = align_term(acc.z, w1, w2, w3, w4, v1.z, v2.z, v3.z, v4.z);
+            acc.w = align_term(acc.w, w1, w2, w3, w4, v1.w, v2.w, v3.w, v4.w);
+          }
+        }
+        if (last) acc = make_float4(__fdiv_rn(acc.x, cnt), __fdiv_rn(acc.y, cnt), __fdiv_rn(acc.z, cnt), __fdiv_rn(acc.w, cnt));
+        reinterpret_cast<float4*>(orow)[i] = acc;
+      }
+    }
+  }
+}
+
+// Max over the bin's cells by '>' from -FLT_MAX in (row, column) order: a NaN never wins, an all-NaN bin gives -FLT_MAX,
+// an empty bin gives 0 (torchvision's roi_pool).
+__global__ void __launch_bounds__(256)
+roi_pool_kernel(const float* __restrict__ feat, int batch, int fh, int fw, int c, const float* __restrict__ rois, int pooled,
+                float scale, float* __restrict__ out) {
+  const int ri = blockIdx.x / pooled, ph = blockIdx.x % pooled;
+  const float* roi = rois + (size_t)ri * 5;
+  const int bi = min(max((int)__ldg(roi), 0), batch - 1);
+  feat += (size_t)bi * fh * fw * c;
+  const int sx = (int)roundf(__fmul_rn(__ldg(roi + 1), scale)), sy = (int)roundf(__fmul_rn(__ldg(roi + 2), scale));
+  const int ex = (int)roundf(__fmul_rn(__ldg(roi + 3), scale)), ey = (int)roundf(__fmul_rn(__ldg(roi + 4), scale));
+  const float bw = __fdiv_rn((float)max(ex - sx + 1, 1), (float)pooled), bh = __fdiv_rn((float)max(ey - sy + 1, 1), (float)pooled);
+  const int h0 = min(max((int)floorf(__fmul_rn((float)ph, bh)) + sy, 0), fh);
+  const int h1 = min(max((int)ceilf(__fmul_rn((float)(ph + 1), bh)) + sy, 0), fh);
+  const int c4 = c >> 2;
+  float* orow = out + (size_t)blockIdx.x * pooled * c;
+  for (int i = threadIdx.x; i < pooled * c4; i += blockDim.x) {
+    const int pw = i / c4, cg = i - pw * c4;
+    const int w0 = min(max((int)floorf(__fmul_rn((float)pw, bw)) + sx, 0), fw);
+    const int w1 = min(max((int)ceilf(__fmul_rn((float)(pw + 1), bw)) + sx, 0), fw);
+    float4 m;
+    if (h1 <= h0 || w1 <= w0) {
+      m = make_float4(0.f, 0.f, 0.f, 0.f);
+    } else {
+      const float lowest = __int_as_float(0xff7fffff);     // -FLT_MAX
+      m = make_float4(lowest, lowest, lowest, lowest);
+      for (int y = h0; y < h1; ++y) {
+        const float4* row = reinterpret_cast<const float4*>(feat + (size_t)y * fw * c) + cg;
+        for (int x = w0; x < w1; ++x) {
+          const float4 v = __ldg(row + (size_t)x * c4);
+          m.x = v.x > m.x ? v.x : m.x; m.y = v.y > m.y ? v.y : m.y; m.z = v.z > m.z ? v.z : m.z; m.w = v.w > m.w ? v.w : m.w;
+        }
+      }
+    }
+    reinterpret_cast<float4*>(orow)[i] = m;
+  }
+}
+
 // ---- RPN decode ---------------------------------------------------------------------------------------------
 __global__ void rpn_decode_kernel(const float* __restrict__ rpn, int ld, int delta_col, const float* __restrict__ base, int A, int batch,
                                   int fh, int fw, int feat_stride, float im_h, float im_w, float* __restrict__ scores,
@@ -580,6 +720,28 @@ extern "C" int frcnn_crop_pool(const float* feat, int batch, int fh, int fw, int
                                float* out, void* stream) {
   FRCNN_REQUIRE(feat && rois && out && batch > 0 && c % 4 == 0 && pooled > 1 && pooled <= CROP_MAX_POOLED, "crop_pool: bad argument");
   crop_pool_kernel<<<(unsigned)(r * pooled), 256, 0, (cudaStream_t)stream>>>(feat, batch, fh, fw, c, rois, r, pooled, pre_pool, out);
+  FRCNN_LAUNCH_CHECK();
+  return OK;
+}
+
+extern "C" int frcnn_roi_align(const float* feat, int batch, int fh, int fw, int c, const float* rois, int r, int pooled,
+                               float spatial_scale, int sampling_ratio, int aligned, float* out, void* stream) {
+  FRCNN_REQUIRE(feat && rois && out && batch > 0 && fh > 0 && fw > 0 && c > 0 && c % 4 == 0 && r >= 0 && pooled >= 1 &&
+                pooled <= ROI_MAX_POOLED && spatial_scale > 0.f && sampling_ratio >= 0 && sampling_ratio <= FRCNN_ROI_ALIGN_MAX_SAMPLING,
+                "roi_align: bad argument");
+  if (r == 0) return OK;
+  roi_align_kernel<<<(unsigned)(r * pooled), 256, 0, (cudaStream_t)stream>>>(feat, batch, fh, fw, c, rois, pooled, spatial_scale,
+                                                                             sampling_ratio, aligned ? 1 : 0, out);
+  FRCNN_LAUNCH_CHECK();
+  return OK;
+}
+
+extern "C" int frcnn_roi_pool(const float* feat, int batch, int fh, int fw, int c, const float* rois, int r, int pooled,
+                              float spatial_scale, float* out, void* stream) {
+  FRCNN_REQUIRE(feat && rois && out && batch > 0 && fh > 0 && fw > 0 && c > 0 && c % 4 == 0 && r >= 0 && pooled >= 1 &&
+                pooled <= ROI_MAX_POOLED && spatial_scale > 0.f, "roi_pool: bad argument");
+  if (r == 0) return OK;
+  roi_pool_kernel<<<(unsigned)(r * pooled), 256, 0, (cudaStream_t)stream>>>(feat, batch, fh, fw, c, rois, pooled, spatial_scale, out);
   FRCNN_LAUNCH_CHECK();
   return OK;
 }

@@ -368,9 +368,16 @@ class ShapePlan(PostStage):
         R = self.R
         # ---- RoI pooling (network.py:141-157 / resnet_v1.py:55-76) ---------------------------------------
         P = cfgd["pooling_size"]
-        pre_pool = net.crop_pre_pool()
         self.pool5 = t.new(B * R, P, P, cb)
-        t.add("crop_pool", lambda: ops.crop_pool(feat, self.rois, P, pre_pool, self.pool5))
+        mode = cfgd["pooling_mode"]
+        if mode == "align":        # extensions: P x P straight from the map, no 2P crop + 2x2 max
+            sr, aligned = cfgd["roi_align"]
+            t.add("roi_align", lambda: ops.roi_align(feat, self.rois, P, SPATIAL_SCALE, sr, aligned, self.pool5))
+        elif mode == "pool":
+            t.add("roi_pool", lambda: ops.roi_pool(feat, self.rois, P, SPATIAL_SCALE, self.pool5))
+        else:
+            pre_pool = net.crop_pre_pool()
+            t.add("crop_pool", lambda: ops.crop_pool(feat, self.rois, P, pre_pool, self.pool5))
         # ---- per-RoI head + fused cls_score|bbox_pred FC (network.py:361-378) ------------------------------
         fc7 = net._head_to_tail(t, self.pool5)
         self.fc7 = fc7
@@ -677,6 +684,47 @@ def check_boxes(boxes, batch):
             raise TypeError("boxes[%d] has dtype %s, expected float32" % (i, a.dtype))
         out.append(np.ascontiguousarray(a))
     return out
+
+
+POOLING_MODES = ("crop", "align", "pool")
+SPATIAL_SCALE = 1.0 / 16     # the stride-16 feature map of every backbone
+
+
+def roi_align_option(pooling_mode, pooling_size, node):
+    """cfg.POOLING_MODE / POOLING_SIZE / ROI_ALIGN -> the network option: None outside 'align' mode, else the checked
+    (SAMPLING_RATIO, ALIGNED).  An unknown mode raises NotImplementedError, an invalid value ValueError, before any device work."""
+    if pooling_mode not in POOLING_MODES:
+        raise NotImplementedError("POOLING_MODE %r: expected one of %s" % (pooling_mode, ", ".join(POOLING_MODES)))
+    if pooling_mode == "crop":
+        return None
+    if type(pooling_size) is not int or not 1 <= pooling_size <= N.ROI_MAX_POOLED:
+        raise ValueError("POOLING_SIZE must be an int in [1, %d] in %r mode, got %r" % (N.ROI_MAX_POOLED, pooling_mode, pooling_size))
+    if pooling_mode == "pool":
+        return None
+    sr, aligned = node["SAMPLING_RATIO"], node["ALIGNED"]
+    if type(sr) is not int or not 0 <= sr <= N.ROI_ALIGN_MAX_SAMPLING:
+        raise ValueError("ROI_ALIGN.SAMPLING_RATIO must be an int in [0, %d] (0 = adaptive), got %r" % (N.ROI_ALIGN_MAX_SAMPLING, sr))
+    if type(aligned) is not bool:
+        raise ValueError("ROI_ALIGN.ALIGNED must be a bool, got %r" % (aligned,))
+    return (sr, aligned)
+
+
+def check_pool_boxes(pooling_mode, boxes, im_scales, blob_hw):
+    """In 'align' and 'pool' mode, refuse caller boxes (original-image pixels) that are not finite or that, scaled into the
+    blob as boxes_to_rois does (fp32 box * fp32 scale), leave [-W, 2W] x [-H, 2H] of the H x W blob: RoIAlign's adaptive
+    grid grows with the box (this keeps it at most about ceil(3 * map size / POOLING_SIZE) per axis), and RoIPool's integer
+    corners must not overflow.  Crop mode takes any box, as before."""
+    if pooling_mode == "crop":
+        return
+    h, w = float(blob_hw[0]), float(blob_hw[1])
+    for i, (a, s) in enumerate(zip(boxes, im_scales)):
+        if not np.isfinite(a).all():
+            raise ValueError("boxes[%d] has a non-finite coordinate (POOLING_MODE %r)" % (i, pooling_mode))
+        r = a * F(s)
+        x, y = r[:, 0::2], r[:, 1::2]
+        if (x < -w).any() or (x > 2 * w).any() or (y < -h).any() or (y > 2 * h).any():
+            raise ValueError("boxes[%d]: in POOLING_MODE %r a box scaled into the %dx%d blob must lie within [-W, 2W] x [-H, 2H]"
+                             % (i, pooling_mode, int(h), int(w)))
 
 
 def check_feature_mode(max_per_image):

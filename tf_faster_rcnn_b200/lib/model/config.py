@@ -75,8 +75,13 @@ cfg = AttrDict(
     EXP_DIR="default",
     USE_GPU_NMS=True,
     USE_E2E_TF=True,
+    # 'crop' (crop_and_resize, the reference's), or the extensions 'align' (RoIAlign, torchvision.ops.roi_align) and 'pool'
+    # (Fast R-CNN's RoIPool, torchvision.ops.roi_pool), which pool straight to POOLING_SIZE x POOLING_SIZE (1..16)
     POOLING_MODE="crop",
     POOLING_SIZE=7,
+    # 'align' mode only: SAMPLING_RATIO int in [0, 16] samples per bin and axis (0 = adaptive, ceil(RoI size / POOLING_SIZE));
+    # ALIGNED: shift the RoI by -0.5 feature cells and drop the minimum size of 1 (Detectron2's RoIAlignV2)
+    ROI_ALIGN=dict(SAMPLING_RATIO=0, ALIGNED=False),
     ANCHOR_SCALES=[8, 16, 32],
     ANCHOR_RATIOS=[0.5, 1, 2],
     RPN_CHANNELS=512,

@@ -131,6 +131,8 @@ def _run_device_preprocess(net, im, post, detect, boxes=None):
     (fp32 [n,4], original-image pixels) instead of the RPN's."""
     from tf_faster_rcnn_b200 import ops, engine
     H, W, f = blob_geometry(im.shape)
+    if boxes is not None:
+        engine.check_pool_boxes(net.options["pooling_mode"], [boxes], [f], (H, W))
     plan = net.plan_for(H, W) if boxes is None else net.plan_for(H, W, cap=engine.box_capacity(boxes.shape[0]))
     img = torch.from_numpy(np.ascontiguousarray(im)).cuda(non_blocking=True)
     ops.preprocess(img, np.asarray(cfg.PIXEL_MEANS, dtype=np.float64).ravel(), f, f, plan.image)

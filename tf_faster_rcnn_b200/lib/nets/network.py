@@ -45,9 +45,10 @@ class Network(object):
         self._num_anchors = self._num_scales * self._num_ratios
         self.base_anchors = generate_anchors(ratios=np.array(self._anchor_ratios), scales=np.array(self._anchor_scales)).astype(np.float32)
         self.anchor_key = "%s|%s" % (self._anchor_scales, self._anchor_ratios)
-        if cfg.POOLING_MODE != "crop":
-            raise NotImplementedError
+        # POOLING_MODE 'crop' (the reference's), 'align' (RoIAlign, with cfg.ROI_ALIGN) or 'pool' (RoIPool); read at plan build
+        roi_align = engine.roi_align_option(cfg.POOLING_MODE, cfg.POOLING_SIZE, cfg.ROI_ALIGN)
         self.options = dict(
+            pooling_mode=cfg.POOLING_MODE, roi_align=roi_align,
             test_mode=cfg.TEST.MODE, use_e2e_tf=bool(cfg.USE_E2E_TF), use_gpu_nms=bool(cfg.USE_GPU_NMS),
             rpn_nms_thresh=cfg.TEST.RPN_NMS_THRESH, rpn_pre_nms_top_n=cfg.TEST.RPN_PRE_NMS_TOP_N,
             rpn_post_nms_top_n=cfg.TEST.RPN_POST_NMS_TOP_N, rpn_top_n=cfg.TEST.RPN_TOP_N,
@@ -232,6 +233,7 @@ class Network(object):
         """Enqueue `images` [B,H,W,3] with caller boxes as the RoIs on a caller-box plan (no sync) -> plan."""
         _no_bbox_aug("caller boxes (score_boxes / im_detect(boxes=))")
         boxes = engine.check_boxes(boxes, int(images.shape[0]))
+        engine.check_pool_boxes(self.options["pooling_mode"], boxes, im_scales, images.shape[1:3])
         plan, meta = self._batch_plan(images, im_scales, orig_hws, cap=engine.box_capacity(max(a.shape[0] for a in boxes)))
         self._copy_in(plan, images)
         plan.set_boxes(boxes)
@@ -241,7 +243,9 @@ class Network(object):
     def score_boxes(self, images, im_scales, orig_hws, boxes):
         """The Fast R-CNN mode: classify and regress caller boxes instead of RPN proposals.  boxes: per image an fp32 [n_i, 4]
         array (x1, y1, x2, y2 in original-image pixels, n_i <= 1024).  -> (list over images of (scores [n_i, C],
-        pred_boxes [n_i, 4C], feats [n_i, F]), plan): im_detect's outputs for those boxes, plus the head features."""
+        pred_boxes [n_i, 4C], feats [n_i, F]), plan): im_detect's outputs for those boxes, plus the head features.
+        With POOLING_MODE 'align' or 'pool', a non-finite box or one that leaves [-W, 2W] x [-H, 2H] of the blob once scaled raises
+        ValueError before any device work."""
         plan = self._run_boxes(images, im_scales, orig_hws, boxes)
         out = []
         for i, a in enumerate(boxes):

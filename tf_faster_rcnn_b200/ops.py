@@ -220,6 +220,20 @@ def crop_pool(feat, rois, pooled, pre_pool, out):
             "crop_pool")
 
 
+def roi_align(feat, rois, pooled, spatial_scale, sampling_ratio, aligned, out):
+    """torchvision.ops.roi_align on NHWC: feat [B,H,W,C], rois [R,5] (image index, x1, y1, x2, y2) -> out [R,pooled,pooled,C]."""
+    b, fh, fw, c = feat.shape
+    N.check(N.lib().frcnn_roi_align(_p(_f32(feat)), b, fh, fw, c, _p(_f32(rois)), rois.shape[0], pooled, float(spatial_scale),
+                                    int(sampling_ratio), int(bool(aligned)), _p(_f32(out)), _stream()), "roi_align")
+
+
+def roi_pool(feat, rois, pooled, spatial_scale, out):
+    """torchvision.ops.roi_pool on NHWC: feat [B,H,W,C], rois [R,5] (image index, x1, y1, x2, y2) -> out [R,pooled,pooled,C]."""
+    b, fh, fw, c = feat.shape
+    N.check(N.lib().frcnn_roi_pool(_p(_f32(feat)), b, fh, fw, c, _p(_f32(rois)), rois.shape[0], pooled, float(spatial_scale),
+                                   _p(_f32(out)), _stream()), "roi_pool")
+
+
 def cls_finish(head_out, num_classes, stds, means, cls_score, cls_prob, bbox_pred):
     r, ld = head_out.shape
     s4 = (C.c_float * 4)(*[float(v) for v in stds])
