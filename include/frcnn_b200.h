@@ -345,6 +345,36 @@ int frcnn_detect_post_soft_vote(const float* cls_prob_dev, const float* pred_box
  * past the count. */
 int frcnn_detect_features(const int* keep_dev, const int* keep_cnt_dev, const float* fc7_dev, int r, int batch, int num_classes,
                           int feat_dim, int max_det, float* feat_out_dev, int* roi_out_dev, void* stream);
+/* Bottom-up regions (Anderson et al. 2018, the protocol of bottom-up-attention's generate_tsv.py), an extension beyond the
+ * reference: per image a set of DISTINCT RoIs, each ranked by its best class confidence after per-class NMS, with its unregressed
+ * box and its head feature.  Per image b, over the valid rows i < nr = min(num_rois[b], r):
+ *   1. box_i = rois[i, 1:5] / scale_b, one fp32 round-to-nearest division per coordinate (scale_b = im_meta[b, 0]; the division of
+ *      frcnn_bbox_decode, no regression, no clipping).
+ *   2. For each class c = 1..C-1: greedy NMS over ALL nr rows (no score threshold) with boxes box_i and scores cls_prob[i, c],
+ *      threshold nms_thresh and predicate `flags` as in frcnn_detect_post; order: score descending, ties to the lower row.
+ *   3. conf_i = max of cls_prob[i, c] over the classes c whose NMS kept i, 0 if none kept it; class_i = the lowest such c reaching
+ *      conf_i, and 0 when conf_i is 0.
+ *   4. count = #{i : conf_i >= conf_thresh}, an fp32 comparison (a caller holding a float64 threshold passes the smallest fp32 not
+ *      below it, which gives the float64 comparison's result for every fp32 conf_i).  If min_boxes <= count <= max_boxes the
+ *      regions are those rows in ascending row order; otherwise the first min(max(count, min_boxes), max_boxes, nr) rows in
+ *      descending conf_i, ties to the lower row.
+ *   5. Region k of image b: boxes_out[b, k] = box_i, conf_out[b, k] = conf_i, class_out[b, k] = class_i, index_out[b, k] = i,
+ *      feat_out[b, k] = fc7 row i; count_out[b] = the number of regions.  Rows k >= count_out[b] are zeros with index -1.
+ * cls_prob entries must be >= +0 (softmax outputs).  Requirements: 2 <= C <= 1024, r <= 8192, conf_thresh in [0, 1],
+ * 0 <= min_boxes <= max_boxes, max_boxes >= 1, feat_dim % 4 == 0.  Buffers (M = min(max_boxes, r)):
+ *   inputs  cls_prob_dev [batch*r, C], rois_dev [batch*r, 5], num_rois_dev int32 [batch], im_meta_dev [batch, 3] (as for
+ *           frcnn_bbox_decode), fc7_dev [batch*r, feat_dim] (16-byte aligned);
+ *   scratch keep_dev / keep_cnt_dev / keep_score_dev and workspace_dev as for frcnn_detect_post (they receive the per-class NMS of
+ *           step 2, uncapped); roi_box_dev [batch*r, C, 4] fp32 (16-byte aligned); key_dev uint64 [batch*r] (8-byte aligned);
+ *   outputs boxes_out_dev [batch, M, 4] (16-byte aligned), conf_out_dev [batch, M], class_out_dev int32 [batch, M], index_out_dev
+ *           int32 [batch, M], feat_out_dev [batch, M, feat_dim] (16-byte aligned), count_out_dev int32 [batch].
+ * No allocation or synchronisation: capturable into a CUDA graph. */
+int frcnn_detect_regions(const float* cls_prob_dev, const float* rois_dev, const int* num_rois_dev, const float* im_meta_dev,
+                         const float* fc7_dev, int r, int batch, int num_classes, int feat_dim, float nms_thresh, unsigned flags,
+                         float conf_thresh, int min_boxes, int max_boxes, int* keep_dev, int* keep_cnt_dev, float* keep_score_dev,
+                         void* workspace_dev, size_t workspace_bytes, float* roi_box_dev, unsigned long long* key_dev,
+                         float* boxes_out_dev, float* conf_out_dev, int* class_out_dev, int* index_out_dev, float* feat_out_dev,
+                         int* count_out_dev, void* stream);
 /* caller boxes -> RoI rows (the Fast R-CNN mode: TEST.HAS_RPN = False).  boxes_dev [batch, cap, 4] fp32 (x1,y1,x2,y2) in
  * ORIGINAL-image pixels; counts_dev int32 [batch]; im_meta_dev [batch, 3] as for frcnn_bbox_decode.  rois_dev [batch*cap, 5] =
  * (b, x1*s, y1*s, x2*s, y2*s), one fp32 multiply by im_meta's scale per coordinate, zeros past the count; num_rois_dev int32

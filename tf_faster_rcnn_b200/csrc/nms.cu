@@ -850,6 +850,129 @@ detect_features_kernel(const int* __restrict__ keep, const int* __restrict__ kee
   }
 }
 
+// ---- bottom-up regions (frcnn_detect_regions; the definition is in include/frcnn_b200.h) -------------------------------------
+// class_nms_kernel runs unchanged over the RoI boxes: roi_box [batch*r, C] holds box_i in every class column, so it reads the RoI
+// box where the post stage reads pred_boxes.  The per-RoI result of all classes is one 64-bit key: the score bits of a kept entry
+// in the high word (scores >= +0, so unsigned order is float order) and ~class in the low word, merged with atomicMax -- the
+// largest score wins and, among equal scores, the lowest class; the result does not depend on the order of the atomics.
+constexpr int REGION_THREADS = 1024;
+constexpr int REGION_CAP = DET_CAP_BIG;   // RoIs per image; the selection sorts up to this many 64-bit keys in shared memory
+
+// thread per (row, class): box_i = rois[row, 1:5] / scale of the row's image, one __fdiv_rn per coordinate (bbox_decode's
+// division); the key of the row is cleared once
+__global__ void regions_boxes_kernel(const float* __restrict__ rois, const float* __restrict__ im_meta, int r, int C, int rows,
+                                     float4* __restrict__ roi_box, unsigned long long* __restrict__ key) {
+  const size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= (size_t)rows * C) return;
+  const int row = (int)(e / C);
+  const float s = __ldg(im_meta + (size_t)(row / r) * 3);
+  const float* q = rois + (size_t)row * 5;
+  roi_box[e] = make_float4(__fdiv_rn(__ldg(q + 1), s), __fdiv_rn(__ldg(q + 2), s), __fdiv_rn(__ldg(q + 3), s), __fdiv_rn(__ldg(q + 4), s));
+  if (e == (size_t)row * C) key[row] = 0ull;
+}
+
+// one CTA per (foreground class, image): folds the class's kept list into the per-RoI keys
+__global__ void regions_fold_kernel(const int* __restrict__ keep, const int* __restrict__ keep_cnt, const float* __restrict__ keep_score,
+                                    int r, int C, unsigned long long* __restrict__ key) {
+  const int cls = blockIdx.x + 1, img = blockIdx.y;
+  const size_t row = ((size_t)img * C + cls) * r;
+  const int nk = __ldg(keep_cnt + (size_t)img * C + cls);
+  for (int j = threadIdx.x; j < nk; j += blockDim.x) {
+    const unsigned long long k = ((unsigned long long)__float_as_uint(__ldg(keep_score + row + j)) << 32) | (unsigned)~cls;
+    atomicMax(key + (size_t)img * r + __ldg(keep + row + j), k);
+  }
+}
+
+// one CTA per image: count conf >= thresh, then either the ascending compaction (min_boxes <= count <= max_boxes) or a bitonic sort
+// of the cap (conf, ~index) keys, descending (conf descending, ties to the lower index); then the outputs of rows [0, max_out).
+// Dynamic shared memory: cap (power of two >= r) 64-bit words.
+__global__ void __launch_bounds__(REGION_THREADS, 1)
+regions_select_kernel(const unsigned long long* __restrict__ key, const float4* __restrict__ roi_box, const int* __restrict__ num_rois,
+                      int r, int C, int cap, float conf_thresh, int min_boxes, int max_boxes, int max_out, float* __restrict__ boxes_out,
+                      float* __restrict__ conf_out, int* __restrict__ class_out, int* __restrict__ index_out, int* __restrict__ count_out) {
+  extern __shared__ __align__(16) unsigned long long sel[];
+  __shared__ int s_warp[REGION_THREADS / 32];
+  constexpr int NW = REGION_THREADS / 32;
+  const int img = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  key += (size_t)img * r;
+  const int nr = max(0, min(__ldg(num_rois + img), r));
+  auto conf_of = [&](int e) { return __uint_as_float((unsigned)(key[e] >> 32)); };
+  int mine = 0;
+  for (int e = tid; e < nr; e += REGION_THREADS) mine += conf_of(e) >= conf_thresh;
+  for (int o = 16; o; o >>= 1) mine += __shfl_xor_sync(0xffffffffu, mine, o);
+  if (lane == 0) s_warp[warp] = mine;
+  __syncthreads();
+  int count = 0;
+  for (int w = 0; w < NW; ++w) count += s_warp[w];
+  __syncthreads();
+  const bool in_range = count >= min_boxes && count <= max_boxes;
+  const int n = in_range ? count : min(min(max(count, min_boxes), max_boxes), nr);
+  if (in_range) {
+    // ordered compaction in windows of REGION_THREADS rows; sel[k] holds ~index in its low word
+    int done = 0;
+    for (int base = 0; base < nr; base += REGION_THREADS) {
+      const int e = base + tid;
+      const bool f = e < nr && conf_of(e) >= conf_thresh;
+      const unsigned bal = __ballot_sync(0xffffffffu, f);
+      if (lane == 0) s_warp[warp] = __popc(bal);
+      __syncthreads();
+      int before = 0, tot = 0;
+      for (int w = 0; w < NW; ++w) { const int v = s_warp[w]; before += w < warp ? v : 0; tot += v; }
+      if (f) sel[done + before + __popc(bal & ((1u << lane) - 1u))] = (unsigned)~e;
+      done += tot;
+      __syncthreads();
+    }
+  } else {
+    for (int e = tid; e < cap; e += REGION_THREADS)
+      sel[e] = e < nr ? (key[e] & 0xffffffff00000000ull) | (unsigned)~e : 0ull;   // the keys are distinct except the padding
+    __syncthreads();
+    for (int k = 2; k <= cap; k <<= 1) {
+      for (int j = k >> 1; j > 0; j >>= 1) {
+        for (int e = tid; e < cap; e += REGION_THREADS) {
+          const int ixj = e ^ j;
+          if (ixj > e) {
+            const unsigned long long a = sel[e], b = sel[ixj];
+            if (((e & k) == 0) ? (a < b) : (a > b)) { sel[e] = b; sel[ixj] = a; }
+          }
+        }
+        __syncthreads();
+      }
+    }
+  }
+  __syncthreads();
+  for (int k = tid; k < max_out; k += REGION_THREADS) {
+    float4 b = make_float4(0.f, 0.f, 0.f, 0.f);
+    float cf = 0.f;
+    int cl = 0, i = -1;
+    if (k < n) {
+      i = (int)~(unsigned)sel[k];
+      const unsigned long long kk = key[i];
+      const unsigned cb = (unsigned)(kk >> 32);
+      cf = __uint_as_float(cb);
+      cl = cb ? (int)~(unsigned)kk : 0;
+      b = roi_box[((size_t)img * r + i) * C];
+    }
+    const size_t o = (size_t)img * max_out + k;
+    reinterpret_cast<float4*>(boxes_out)[o] = b;
+    conf_out[o] = cf; class_out[o] = cl; index_out[o] = i;
+  }
+  if (tid == 0) count_out[img] = n;
+}
+
+// one CTA per (block of FEAT_SLOTS output rows, image): fc7 row of each selected RoI, zeros past the count
+__global__ void __launch_bounds__(FEAT_THREADS)
+regions_features_kernel(const int* __restrict__ index_out, const float4* __restrict__ fc7, int r, int f4, int max_out,
+                        float4* __restrict__ feat_out) {
+  const int img = blockIdx.y, k0 = blockIdx.x * FEAT_SLOTS;
+  const float4* src = fc7 + (size_t)img * r * f4;
+  for (int t = threadIdx.x; t < FEAT_SLOTS * f4; t += FEAT_THREADS) {
+    const int s = t / f4, q = t - s * f4, k = k0 + s;
+    if (k >= max_out) break;
+    const int i = __ldg(index_out + (size_t)img * max_out + k);
+    feat_out[((size_t)img * max_out + k) * f4 + q] = i >= 0 ? __ldg(src + (size_t)i * f4 + q) : make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+}
+
 }  // namespace frcnn
 
 using namespace frcnn;
@@ -1011,6 +1134,25 @@ static int detect_post_run(const char* who, const float* cls_prob, const float* 
   return OK;
 }
 
+// the greedy per-class NMS launch of the post entries and frcnn_detect_regions: the kept sets in shared memory up to DET_CAP RoIs,
+// else in `workspace`
+static int class_nms_launch(dim3 grid, cudaStream_t st, const float* cls_prob, const float4* pred, const int* num_rois, int r, int batch,
+                            int num_classes, float score_thresh, float nms_thresh, unsigned flags, int* keep, int* keep_cnt,
+                            float* keep_score, void* workspace, size_t workspace_bytes) {
+  if (r <= DET_CAP) {
+    class_nms_kernel<DET_CAP, false><<<grid, NMS_THREADS, DET_CAP * 32, st>>>(cls_prob, pred, num_rois, r, num_classes, score_thresh,
+                                                                              nms_thresh, flags, keep, keep_cnt, keep_score, nullptr);
+    return OK;
+  }
+  FRCNN_REQUIRE(workspace && workspace_bytes >= frcnn_detect_post_workspace_bytes(r, num_classes, batch), "detect_post: workspace too small");
+  static bool attr_done[MAX_DEVICES];
+  if (int rc = smem_attr_once(class_nms_kernel<DET_CAP_BIG, true>, DET_CAP_BIG * 8, attr_done)) return rc;
+  class_nms_kernel<DET_CAP_BIG, true><<<grid, NMS_THREADS, DET_CAP_BIG * 8, st>>>(cls_prob, pred, num_rois, r, num_classes, score_thresh,
+                                                                                  nms_thresh, flags, keep, keep_cnt, keep_score,
+                                                                                  reinterpret_cast<uint8_t*>(workspace));
+  return OK;
+}
+
 // the greedy post (frcnn_detect_post / _vote); vote == nullptr: no voting stage
 static int greedy_post(const char* who, const float* cls_prob, const float* pred_boxes, const int* num_rois, int r, int batch,
                        int num_classes, float score_thresh, float nms_thresh, unsigned flags, int max_per_image, int max_det, float* det,
@@ -1019,18 +1161,8 @@ static int greedy_post(const char* who, const float* cls_prob, const float* pred
   return detect_post_run(who, cls_prob, pred_boxes, num_rois, r, batch, num_classes, score_thresh, max_per_image, max_det, det,
                          ndet, record_stride, keep, keep_cnt, keep_score, vote, vote_box, stream,
                          [&](dim3 grid, cudaStream_t st, const float4* pred) -> int {
-    if (r <= DET_CAP) {
-      class_nms_kernel<DET_CAP, false><<<grid, NMS_THREADS, DET_CAP * 32, st>>>(cls_prob, pred, num_rois, r, num_classes, score_thresh,
-                                                                                nms_thresh, flags, keep, keep_cnt, keep_score, nullptr);
-      return OK;
-    }
-    FRCNN_REQUIRE(workspace && workspace_bytes >= frcnn_detect_post_workspace_bytes(r, num_classes, batch), "detect_post: workspace too small");
-    static bool attr_done[MAX_DEVICES];
-    if (int rc = smem_attr_once(class_nms_kernel<DET_CAP_BIG, true>, DET_CAP_BIG * 8, attr_done)) return rc;
-    class_nms_kernel<DET_CAP_BIG, true><<<grid, NMS_THREADS, DET_CAP_BIG * 8, st>>>(cls_prob, pred, num_rois, r, num_classes, score_thresh,
-                                                                                    nms_thresh, flags, keep, keep_cnt, keep_score,
-                                                                                    reinterpret_cast<uint8_t*>(workspace));
-    return OK;
+    return class_nms_launch(grid, st, cls_prob, pred, num_rois, r, batch, num_classes, score_thresh, nms_thresh, flags, keep, keep_cnt,
+                            keep_score, workspace, workspace_bytes);
   });
 }
 
@@ -1194,6 +1326,49 @@ extern "C" int frcnn_detect_features(const int* keep, const int* keep_cnt, const
   detect_features_kernel<<<grid, FEAT_THREADS, 0, (cudaStream_t)stream>>>(keep, keep_cnt, reinterpret_cast<const float4*>(fc7), r,
                                                                          num_classes, feat_dim / 4, max_det,
                                                                          reinterpret_cast<float4*>(feat_out), roi_out);
+  FRCNN_LAUNCH_CHECK();
+  return OK;
+}
+
+extern "C" int frcnn_detect_regions(const float* cls_prob, const float* rois, const int* num_rois, const float* im_meta, const float* fc7,
+                                    int r, int batch, int num_classes, int feat_dim, float nms_thresh, unsigned flags, float conf_thresh,
+                                    int min_boxes, int max_boxes, int* keep, int* keep_cnt, float* keep_score, void* workspace,
+                                    size_t workspace_bytes, float* roi_box, unsigned long long* key, float* boxes_out, float* conf_out,
+                                    int* class_out, int* index_out, float* feat_out, int* count_out, void* stream) {
+  FRCNN_REQUIRE(cls_prob && rois && num_rois && im_meta && fc7 && keep && keep_cnt && keep_score && roi_box && key && boxes_out &&
+                conf_out && class_out && index_out && feat_out && count_out, "detect_regions: null pointer");
+  FRCNN_REQUIRE(r > 0 && batch > 0 && num_classes >= 2 && num_classes <= 1024, "detect_regions: r>0, batch>0, 2<=C<=1024 required");
+  if (r > REGION_CAP) { set_error("detect_regions: %d RoIs per image > capacity %d", r, REGION_CAP); return ERR_CAPACITY; }
+  FRCNN_REQUIRE(feat_dim > 0 && feat_dim % 4 == 0 && ((uintptr_t)fc7 & 15) == 0 && ((uintptr_t)feat_out & 15) == 0,
+                "detect_regions: feat_dim %d must be a positive multiple of 4 and fc7 / feat_out 16-byte aligned", feat_dim);
+  FRCNN_REQUIRE(((uintptr_t)roi_box & 15) == 0 && ((uintptr_t)boxes_out & 15) == 0 && ((uintptr_t)key & 7) == 0,
+                "detect_regions: roi_box / boxes_out must be 16-byte and key 8-byte aligned");
+  FRCNN_REQUIRE(conf_thresh >= 0.f && conf_thresh <= 1.f, "detect_regions: conf_thresh must lie in [0, 1]");
+  FRCNN_REQUIRE(min_boxes >= 0 && max_boxes >= 1 && min_boxes <= max_boxes, "detect_regions: 0 <= min_boxes <= max_boxes, max_boxes >= 1 required");
+  FRCNN_REQUIRE(r <= DET_CAP || (workspace && workspace_bytes >= frcnn_detect_post_workspace_bytes(r, num_classes, batch)),
+                "detect_regions: workspace too small");
+  cudaStream_t st = (cudaStream_t)stream;
+  float4* rb = reinterpret_cast<float4*>(roi_box);
+  const int rows = r * batch;
+  regions_boxes_kernel<<<(unsigned)(((size_t)rows * num_classes + 255) / 256), 256, 0, st>>>(rois, im_meta, r, num_classes, rows, rb, key);
+  FRCNN_LAUNCH_CHECK();
+  // every valid row is a candidate of every class: score_thresh -1 < any score >= +0
+  if (int rc = class_nms_launch(dim3((unsigned)(num_classes - 1), (unsigned)batch), st, cls_prob, rb, num_rois, r, batch, num_classes, -1.f,
+                                nms_thresh, flags, keep, keep_cnt, keep_score, workspace, workspace_bytes)) return rc;
+  FRCNN_LAUNCH_CHECK();
+  regions_fold_kernel<<<dim3((unsigned)(num_classes - 1), (unsigned)batch), 256, 0, st>>>(keep, keep_cnt, keep_score, r, num_classes, key);
+  FRCNN_LAUNCH_CHECK();
+  int cap = 1;
+  while (cap < r) cap <<= 1;
+  static bool attr_done[MAX_DEVICES];
+  if (int rc = smem_attr_once(regions_select_kernel, (size_t)REGION_CAP * 8, attr_done)) return rc;
+  const int max_out = max_boxes < r ? max_boxes : r;
+  regions_select_kernel<<<(unsigned)batch, REGION_THREADS, (size_t)cap * 8, st>>>(key, rb, num_rois, r, num_classes, cap, conf_thresh,
+                                                                                  min_boxes, max_boxes, max_out, boxes_out, conf_out,
+                                                                                  class_out, index_out, count_out);
+  FRCNN_LAUNCH_CHECK();
+  regions_features_kernel<<<dim3((unsigned)cdiv(max_out, FEAT_SLOTS), (unsigned)batch), FEAT_THREADS, 0, st>>>(
+      index_out, reinterpret_cast<const float4*>(fc7), r, feat_dim / 4, max_out, reinterpret_cast<float4*>(feat_out));
   FRCNN_LAUNCH_CHECK();
   return OK;
 }

@@ -224,6 +224,9 @@ REC_HEADER = 8     # 4-byte words in front of every image's detection rows: word
 # the options the post step is built for; a change rebuilds it (PostStage._ensure_post).  soft_nms: soft_nms_args() or None;
 # box_vote: box_vote_args() or None
 PostKey = collections.namedtuple("PostKey", "score_thresh nms_thresh use_gpu_nms max_per_image soft_nms box_vote", defaults=(None,))
+# the options the bottom-up regions step is built for (PostStage._ensure_regions); conf_thresh is the fp32 threshold of region_args
+RegionKey = collections.namedtuple("RegionKey", "conf_thresh min_boxes max_boxes nms_thresh use_gpu_nms")
+REGION_FIELDS = ("boxes", "features", "conf", "classes", "roi_index")
 
 
 class PostStage:
@@ -231,12 +234,15 @@ class PostStage:
     rows): the per-class NMS or Soft-NMS into `keep` / `keep_cnt` / `keep_score` (`post_ws`: the greedy NMS's workspace), with
     the box_vote option the voting into `vote_box`, the max_per_image cap and the detection records, built on first use for the
     options in force; in feature mode also the
-    per-detection gather of `fc7`.  The subclass allocates those buffers.  Two record buffers: with `double_buffer`,
+    per-detection gather of `fc7`; in region mode the bottom-up regions step over `cls_prob`, `rois`, `num_rois`, `im_meta` and
+    `fc7`.  The subclass allocates those buffers.  Two record buffers: with `double_buffer`,
     consecutive detect launches alternate between them.  Also the plan's CUDA-graph cache."""
 
     def __init__(self, net, batch, use_graph):
         self.net, self.batch = net, batch
         self.post_key = None
+        self.regions_key = self.regions_step = None                 # region mode (_ensure_regions)
+        self.reg_box = self.reg_key = self.reg_out = None
         self.recs = [None, None]
         self.rec = self.ndet = None    # views of the buffer the LAST detect launch wrote
         self.post_steps = [None, None]
@@ -292,6 +298,40 @@ class PostStage:
         self.graphs.pop(("detect", 0), None); self.graphs.pop(("detect", 1), None)
         self.feat_out = self.roi_out = self.features_step = None
         self.graphs.pop(("features", 0), None)
+
+    def _ensure_regions(self, conf_thresh, min_boxes, max_boxes):
+        """(Re)build the bottom-up regions step for region_args' (fp32 conf_thresh, min_boxes, max_boxes) and the NMS options in
+        force.  Its buffers are allocated on first use: the RoI boxes broadcast over the classes, the per-RoI keys and
+        min(max_boxes, R) output rows per image; the per-class NMS reuses keep / keep_cnt / keep_score / post_ws."""
+        o = self.net.options
+        key = RegionKey(float(conf_thresh), int(min_boxes), int(max_boxes), float(o["nms_thresh"]), bool(o["use_gpu_nms"]))
+        if key == self.regions_key:
+            return
+        C, R, B = self.net.num_classes, self.R, self.batch
+        if self.reg_box is None:
+            self.reg_box = ops.zeros((B * R, C, 4))
+            self.reg_key = ops.zeros((B * R,), dtype=torch.int64)
+        M = min(key.max_boxes, R)
+        if self.reg_out is None or self.reg_out["conf"].shape[1] != M:
+            fdim = int(self.fc7.shape[1])
+            self.reg_out = dict(boxes=ops.zeros((B, M, 4)), features=ops.zeros((B, M, fdim)), conf=ops.zeros((B, M)),
+                                classes=ops.zeros((B, M), dtype=torch.int32), roi_index=ops.zeros((B, M), dtype=torch.int32),
+                                count=ops.zeros((B,), dtype=torch.int32))
+        thr, flags = nms_threshold(key.nms_thresh, key.use_gpu_nms)
+        out = self.reg_out
+        self.regions_step = lambda: ops.detect_regions(self.cls_prob, self.rois, self.num_rois, self.im_meta, self.fc7, C, thr, flags,
+                                                       key.conf_thresh, key.min_boxes, key.max_boxes, self.keep, self.keep_cnt,
+                                                       self.keep_score, self.post_ws, self.reg_box, self.reg_key, out, batch=B)
+        for g in [g for g in self.graphs if isinstance(g, tuple) and g[0] == "regions"]:
+            del self.graphs[g]
+        self.regions_key = key
+
+    def regions(self):
+        """Host copy of the bottom-up regions of the batch after a 'regions' launch: per image a dict of boxes [n,4] fp32,
+        features [n,F] fp32, conf [n] fp32, classes [n] int32, roi_index [n] int32."""
+        host = {k: v.cpu() for k, v in self.reg_out.items()}
+        counts = host["count"].numpy()
+        return [{k: host[k][b, :int(counts[b])].numpy().copy() for k in REGION_FIELDS} for b in range(self.batch)]
 
     def _select(self, slot):
         self.slot = slot
@@ -484,12 +524,16 @@ class ShapePlan(PostStage):
         self.recs = [None, None]
         self.rec = self.ndet = None
         self.feat_out = self.roi_out = self.features_step = None
+        self.regions_key = self.regions_step = None
+        self.reg_box = self.reg_key = self.reg_out = None
 
     def steps_for(self, mode):
         """mode: 'test_image' (network outputs), 'im_detect' (+ decoded boxes), 'detect' (+ per-class NMS, cap, records),
-        'features' (+ the head feature and RoI index of every record row); the last two after _begin_post."""
-        if mode == "test_image":
-            return [fn for _, fn in self.tape.steps[:self.n_test_image_steps]]
+        'features' (+ the head feature and RoI index of every record row); the last two after _begin_post.  'regions': the
+        network outputs + the bottom-up regions step (no box decode, no records), after _ensure_regions."""
+        if mode in ("test_image", "regions"):
+            fns = [fn for _, fn in self.tape.steps[:self.n_test_image_steps]]
+            return fns + [self.regions_step] if mode == "regions" else fns
         fns = [fn for _, fn in self.tape.steps[:self.n_im_detect_steps]]
         if mode in ("detect", "features"):
             fns.append(self.post_steps[self.slot])
@@ -505,11 +549,12 @@ class ShapePlan(PostStage):
             host[b, 0] = float(F(s)); host[b, 1] = float(oh); host[b, 2] = float(ow)
         self.im_meta.copy_(host, non_blocking=True)
 
-    def launch(self, im_scale=1.0, orig_h=None, orig_w=None, post=False, detect=False, meta=None, features=False):
+    def launch(self, im_scale=1.0, orig_h=None, orig_w=None, post=False, detect=False, meta=None, features=False, regions=None):
         """Enqueue one batch (inputs already in self.image) on the current stream.  meta: per-image (scale, orig_h, orig_w)
         rows; the scalar arguments describe every image of the batch when meta is None.  features: detect + the feature
-        gather into feat_out / roi_out (always record buffer 0: feature mode does not double-buffer)."""
-        mode = "features" if features else "detect" if detect else ("im_detect" if post else "test_image")
+        gather into feat_out / roi_out (always record buffer 0: feature mode does not double-buffer).  regions: region_args'
+        (conf_thresh, min_boxes, max_boxes) -> the network outputs + the bottom-up regions into reg_out (see regions())."""
+        mode = "regions" if regions is not None else "features" if features else "detect" if detect else ("im_detect" if post else "test_image")
         if mode != "test_image":
             if meta is None:
                 meta = [(im_scale, orig_h if orig_h is not None else self.h, orig_w if orig_w is not None else self.w)] * self.batch
@@ -518,6 +563,9 @@ class ShapePlan(PostStage):
         if mode in ("detect", "features"):
             self._begin_post(features)
             gkey = (mode, self.slot)
+        elif mode == "regions":
+            self._ensure_regions(*regions)
+            gkey = ("regions", self.regions_key)
         self._replay(gkey, self.steps_for(mode))
 
 
@@ -727,6 +775,34 @@ def check_pool_boxes(pooling_mode, boxes, im_scales, blob_hw):
                              % (i, pooling_mode, int(h), int(w)))
 
 
+def f32_not_below(t):
+    """The smallest fp32 value >= the float64 t: for every fp32 x, x >= t (in float64) <=> x >= f32_not_below(t) (in fp32)."""
+    t32 = F(t)
+    if float(t32) < float(t):
+        t32 = np.nextafter(t32, F(np.inf))
+    return t32
+
+
+def _is_int(v):
+    return isinstance(v, (int, np.integer)) and not isinstance(v, (bool, np.bool_))
+
+
+def region_args(conf_thresh, min_boxes, max_boxes):
+    """Bottom-up region parameters -> (fp32 conf threshold: the smallest fp32 not below conf_thresh, min_boxes, max_boxes);
+    raises ValueError before any device work."""
+    try:
+        t = float(conf_thresh)
+    except (TypeError, ValueError):
+        raise ValueError("conf_thresh must be a number in [0, 1], got %r" % (conf_thresh,))
+    if isinstance(conf_thresh, (bool, np.bool_)) or not np.isfinite(t) or not 0.0 <= t <= 1.0:
+        raise ValueError("conf_thresh must be a finite number in [0, 1], got %r" % (conf_thresh,))
+    if not (_is_int(min_boxes) and _is_int(max_boxes)):
+        raise ValueError("min_boxes / max_boxes must be integers, got %r / %r" % (min_boxes, max_boxes))
+    if min_boxes < 0 or max_boxes < 1 or min_boxes > max_boxes:
+        raise ValueError("need 0 <= min_boxes <= max_boxes and max_boxes >= 1, got min_boxes %d, max_boxes %d" % (min_boxes, max_boxes))
+    return float(f32_not_below(t)), int(min_boxes), int(max_boxes)
+
+
 def check_feature_mode(max_per_image):
     if max_per_image <= 0:
         raise ValueError("per-detection features need max_per_image > 0: without the cap the record buffer holds every "
@@ -777,9 +853,6 @@ def nms_threshold(thresh, use_gpu_nms):
     """(fp32 threshold, flags) reproducing the reference's two '+1' predicates:
     cpu_nms compares the fp32 overlap with a DOUBLE threshold using >= (cpu_nms.pyx:17,65)  <=> ovr >= ceil32(t);
     gpu_nms compares with float(t) using > (nms_kernel.cu:34,71)."""
-    t32 = F(thresh)
     if use_gpu_nms:
-        return float(t32), N.NMS_MODE_GPU_NMS
-    if float(t32) < float(thresh):
-        t32 = np.nextafter(t32, F(np.inf))
-    return float(t32), N.NMS_MODE_CPU_NMS
+        return float(F(thresh)), N.NMS_MODE_GPU_NMS
+    return float(f32_not_below(thresh)), N.NMS_MODE_CPU_NMS

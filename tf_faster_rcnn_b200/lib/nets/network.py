@@ -229,6 +229,22 @@ class Network(object):
         feats, rois = plan.feat_out.cpu(), plan.roi_out.cpu()
         return [(d, feats[i, :d.shape[0]].numpy().copy(), rois[i, :d.shape[0]].numpy().copy()) for i, d in enumerate(dets)], plan
 
+    def detect_regions(self, images, im_scales, orig_hws, conf_thresh=0.2, min_boxes=10, max_boxes=100):
+        """Bottom-up regions (Anderson et al. 2018, bottom-up-attention's generate_tsv.py): per image the distinct RoIs ranked by
+        their best class confidence after per-class NMS over all RoIs (TEST.NMS, USE_GPU_NMS's predicate), the RoIs with
+        confidence >= conf_thresh in ascending RoI order when there are min_boxes to max_boxes of them, else the top
+        min(max(count, min_boxes), max_boxes) by confidence.  One graph replay after the network outputs; the definition is
+        frcnn_detect_regions' (include/frcnn_b200.h).  TEST.SOFT_NMS, TEST.BBOX_VOTE and max_per_image do not apply.
+        -> (list over images of dict(boxes [n,4] fp32 unregressed RoI boxes in image pixels, features [n,F] fp32, conf [n] fp32,
+        classes [n] int32, roi_index [n] int32), plan).  ValueError before any device work for a conf_thresh outside [0, 1], counts
+        that are not integers with 0 <= min_boxes <= max_boxes, max_boxes >= 1, and with TEST.BBOX_AUG enabled."""
+        _no_bbox_aug("bottom-up regions (detect_regions)")
+        args = engine.region_args(conf_thresh, min_boxes, max_boxes)
+        plan, meta = self._batch_plan(images, im_scales, orig_hws)
+        self._copy_in(plan, images)
+        plan.launch(meta=meta, regions=args)
+        return plan.regions(), plan
+
     def _run_boxes(self, images, im_scales, orig_hws, boxes):
         """Enqueue `images` [B,H,W,3] with caller boxes as the RoIs on a caller-box plan (no sync) -> plan."""
         _no_bbox_aug("caller boxes (score_boxes / im_detect(boxes=))")

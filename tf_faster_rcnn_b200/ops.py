@@ -315,6 +315,21 @@ def detect_features(keep, keep_cnt, fc7, num_classes, feat_out, roi_out):
                                           _p(roi_out), _stream()), "detect_features")
 
 
+def detect_regions(cls_prob, rois, num_rois, im_meta, fc7, num_classes, nms_thresh, flags, conf_thresh, min_boxes, max_boxes, keep,
+                   keep_cnt, keep_score, workspace, roi_box, key, out, batch=1):
+    """Bottom-up regions (frcnn_detect_regions): cls_prob [batch*r, C], rois [batch*r, 5], num_rois int32 [batch], im_meta
+    [batch, 3], fc7 [batch*r, F]; keep / keep_cnt / keep_score / workspace as for detect_post; roi_box [batch*r, C, 4] fp32 and
+    key int64 [batch*r] scratch.  out: dict of boxes [batch, M, 4], conf [batch, M], classes int32 [batch, M], roi_index int32
+    [batch, M], features [batch, M, F], count int32 [batch] with M = min(max_boxes, r).  conf_thresh is the fp32 threshold."""
+    r = cls_prob.shape[0] // batch
+    fdim = fc7.shape[1]
+    N.check(N.lib().frcnn_detect_regions(_p(_f32(cls_prob)), _p(_f32(rois)), _p(num_rois), _p(_f32(im_meta)), _p(_f32(fc7)), r, batch,
+                                         num_classes, fdim, float(nms_thresh), flags, float(conf_thresh), int(min_boxes), int(max_boxes),
+                                         _p(keep), _p(keep_cnt), _p(keep_score), _p(workspace), 0 if workspace is None else workspace.numel(),
+                                         _p(_f32(roi_box)), _p(key), _p(_f32(out["boxes"])), _p(_f32(out["conf"])), _p(out["classes"]),
+                                         _p(out["roi_index"]), _p(_f32(out["features"])), _p(out["count"]), _stream()), "detect_regions")
+
+
 def boxes_to_rois(boxes, counts, im_meta, rois, num_rois):
     """boxes [batch, cap, 4] original-image pixels, counts int32 [batch], im_meta [batch, 3] -> rois [batch*cap, 5], num_rois."""
     batch, cap, _ = boxes.shape
