@@ -39,6 +39,7 @@ import numpy as np
 
 import conv_split_model as M
 import front_ref64 as FR
+import fused_ref64 as R
 import stage_ref64 as S
 from oracle import nets as ON
 
@@ -304,11 +305,14 @@ def conv_ref(lay, w, xs, mode, pos):
     concat = len(parts) > 1
     whi_parts = None
     if concat and mode == M.F16X1:
-        # F16X1's operand model of a projection unit: the device packs [W_1 inv32_1 ; W_2 inv32_2] (fp32 products,
-        # engine.concat_layers) with ONE weight exponent for the whole matrix, so the split is taken on that matrix
-        packed = np.concatenate([(wt * fold32(w, nm, p["eps"])[0]).astype(F) for (_, wt, *_), nm in zip(parts, p["parts"])],
+        # F16X1's operand model of a projection unit: the device packs W' = [W_1 inv32_1 ; W_2 inv32_2] (fp32 products,
+        # engine.concat_layers) as W' / sigma (sigma: a power of two per column, fused_ref64.pack_columns) with ONE weight
+        # exponent for the whole matrix and multiplies by sigma in the epilogue, so the split is taken on that matrix
+        folded = np.concatenate([(wt * fold32(w, nm, p["eps"])[0]).astype(F) for (_, wt, *_), nm in zip(parts, p["parts"])],
                                 axis=2)
+        packed, sigma = R.pack_columns(folded)
         whi, _ = M.split_weights(packed.reshape(-1, packed.shape[-1]), M.F16X1)
+        whi = whi * sigma.astype(np.float64)
         cuts = np.cumsum([0] + [q[1].shape[2] for q in parts])
         whi_parts = [whi[cuts[j]:cuts[j + 1]] for j in range(len(parts))]
     a = np.zeros((len(pos), parts[0][1].shape[-1]))
@@ -518,7 +522,8 @@ def standin(layers, w, image, mode=M.F16X3, mutant=None, tile=(8, 16)):
         elif len(p["parts"]) > 1:
             parts = [fold32(w, nm, eps) for nm in p["parts"]]
             wt = np.concatenate([(np.asarray(w[nm + "/weights"], F) * s).astype(F) for nm, (s, _) in zip(p["parts"], parts)], axis=2)
-            sc, sh = None, (parts[0][1] + parts[1][1]).astype(F)
+            wt, sc = R.pack_columns(wt)                                  # engine.concat_layers' packing
+            sh = (parts[0][1] + parts[1][1]).astype(F)
         else:
             wt = np.asarray(w[p["name"] + "/weights"], F)
             sc, sh = fold32(w, p["name"], eps)

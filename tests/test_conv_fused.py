@@ -22,6 +22,7 @@ import pytest
 import torch
 
 import conv_split_model as M
+import fused_ref64 as R
 import stage_ref64 as S
 
 F = np.float32
@@ -49,7 +50,9 @@ class _W(dict):
         return engine.bn_fold(self[p + "gamma"], self[p + "beta"], self[p + "moving_mean"], self[p + "moving_variance"], bn_eps)
 
 
-def test_concat_layers_folds_scales_in_fp32():
+def test_concat_layers_folds_scales_in_fp32_per_column_pow2():
+    """The BatchNorm scales are folded into the weights in fp32 (w * sigma == the numpy fp32 products, bit for bit), each
+    output column packed by a power of two sigma that returns as the epilogue scale, and the shifts summed in fp32."""
     from tf_faster_rcnn_b200 import engine, ops
     rng = np.random.default_rng(11)
     t = _W()
@@ -61,12 +64,16 @@ def test_concat_layers_folds_scales_in_fp32():
     w, sc, sh = engine.concat_layers(t, ["a/conv3", "a/shortcut"], 1e-5)
     s3, b3 = t.scale_shift("a/conv3", 1e-5)
     ssc, bsc = t.scale_shift("a/shortcut", 1e-5)
-    assert sc is None and w.dtype == F and sh.dtype == F and w.shape == (1, 1, 160, 256)
-    want = np.concatenate([t["a/conv3/weights"] * s3, t["a/shortcut/weights"] * ssc], axis=2)   # fp32 products, numpy
-    assert np.array_equal(w.view(np.int32), want.astype(F).view(np.int32))
+    assert sc.dtype == F and w.dtype == F and sh.dtype == F and w.shape == (1, 1, 160, 256) and sc.shape == (256,)
+    want = np.concatenate([t["a/conv3/weights"] * s3, t["a/shortcut/weights"] * ssc], axis=2).astype(F)   # fp32 products
+    # packed per output column: W' / sigma with sigma a power of two, so w * sigma gives the fp32 products back exactly
+    assert (np.frexp(sc)[0] == 0.5).all()
+    assert np.array_equal((w * sc).astype(F).view(np.int32), want.view(np.int32))
+    m = np.abs(w).reshape(-1, 256).max(axis=0)
+    assert ((m >= 1) & (m < 2)).all()
     assert np.array_equal(sh.view(np.int32), (b3 + bsc).astype(F).view(np.int32))
-    # one weight exponent for the whole matrix: the larger part's
-    assert ops.weight_exponent(w) == min(ops.weight_exponent(w[:, :, :64]), ops.weight_exponent(w[:, :, 64:]))
+    # one weight exponent for the whole matrix, and every column reaches its top binade
+    assert ops.weight_exponent(w) == 13
     # no scale: the weights pass unchanged
     assert np.array_equal(ops.concat_scaled_weights([w[:, :, :64], w[:, :, 64:]], [None, None]), w)
 
@@ -128,8 +135,9 @@ def test_concat_conv_within_bound_of_unfused(cuda, case, mode, block_n):
     s3, ssc = rng.uniform(0.3, 1.5, cout).astype(F), rng.uniform(0.3, 1.5, cout).astype(F)
     b3, bsc = rng.standard_normal(cout).astype(F), rng.standard_normal(cout).astype(F)
     wcat = ops.concat_scaled_weights([w3, wsc], [s3, ssc])
+    wpack, sigma = R.pack_columns(wcat)                   # engine.concat_layers' packing
     shift = (b3 + bsc).astype(F)
-    pc = ops.PackedConv(wcat, None, shift, impl=impl)
+    pc = ops.PackedConv(wpack, sigma, shift, impl=impl)
     hd, xd = dev(h2), dev(x)
     buf, out = S.guarded_out((n, h, w, cout))
     plan = ops.ConvPlan(hd, pc, out, 1, 0, 0, N.ACT_RELU, None, block_n, 0, split_k, x2=xd)
@@ -155,7 +163,7 @@ def test_concat_conv_within_bound_of_unfused(cuda, case, mode, block_n):
         bound = (ALPHA + 2) * U * s + U * np.abs(b3.astype(np.float64) + bsc) + 2 * U * np.abs(pre64)
         alpha_s = ALPHA
     else:
-        m, s = M.model(np.concatenate([h2, x], axis=3), wcat, impl, 1, 0, 0, h, w)
+        m, s = R.folded_model(np.concatenate([h2, x], axis=3), wpack, sigma, impl)
         pre64 = m + shift.astype(np.float64)
         bound = BETA * U * s + 2 * U * np.abs(pre64)
         alpha_s = BETA

@@ -30,14 +30,22 @@ def bn_fold(gamma, beta, mean, var, eps):
 
 
 def concat_layers(weights, names, bn_eps):
-    """(w, scale, shift) of Weights.packed_concat on the host: w = [W_1 diag(s_1) ; ...] fp32, scale None, shift = the shifts
-    added in order in fp32."""
+    """(w, scale, shift) of Weights.packed_concat on the host: W' = [W_1 diag(s_1) ; ...] in fp32, packed as w = W' / sigma
+    with scale = sigma, the power of two per output channel that puts the column's largest |w| in [1, 2)
+    (ops.column_scales); shift = the shifts added in order in fp32.
+
+    Folding the BatchNorm scales moves them from the epilogue into the weights, so without sigma a channel whose scales
+    are both small would sit far below the matrix's largest weight and lose the fp32 grade of the f16 split (it keeps 27
+    binades below the layer's largest weight, ops.weight_exponent).  w * sigma == W' bit for bit (up to weights more than
+    126 binades below their column's largest, whose quotient is subnormal and which the split drops anyway), and the
+    epilogue's scale sigma * out_mult is a power of two, so the device multiplies by it exactly."""
     ss = [weights.scale_shift(nm, bn_eps) for nm in names]
     w = ops.concat_scaled_weights([weights[nm + "/weights"] for nm in names], [s for s, _ in ss])
+    sigma = ops.column_scales(w)
     shift = ss[0][1]
     for _, sh in ss[1:]:
         shift = (shift + sh).astype(F)
-    return w, None, shift
+    return (w / sigma).astype(F), sigma, shift
 
 
 class Weights:
@@ -75,8 +83,8 @@ class Weights:
 
     def packed_concat(self, names, bn_eps):
         """One 1x1 layer computing the sum of the BatchNorm'd 1x1 layers `names` over their concatenated inputs:
-        weights [W_1 diag(s_1) ; W_2 diag(s_2) ; ...] (scales folded in fp32, one weight exponent for the whole matrix),
-        epilogue scale 1 and shift = the sum of the shifts in fp32."""
+        weights [W_1 diag(s_1) ; W_2 diag(s_2) ; ...] (scales folded in fp32, each output column normalised by a power of
+        two that returns as its epilogue scale: concat_layers) and shift = the sum of the shifts in fp32."""
         key = "+".join(names)
         if key not in self._packed:
             self._packed[key] = ops.PackedConv(*concat_layers(self, names, bn_eps))

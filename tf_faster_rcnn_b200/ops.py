@@ -93,6 +93,16 @@ def concat_scaled_weights(ws, scales):
     return np.ascontiguousarray(np.concatenate(parts, axis=2))
 
 
+def column_scales(w):
+    """Per output channel (last axis) the power of two sigma_c with max_k |w[..., c]| / sigma_c in [1, 2); 1 for a column
+    that is all zero or holds a non-finite value.  Dividing a column by its sigma_c and multiplying the epilogue scale by it
+    are both exact, and every column then spans the same binades of the f16 split as the layer's largest weight."""
+    m = np.max(np.abs(np.asarray(w, np.float32)).reshape(-1, w.shape[-1]), axis=0) if w.size else np.zeros(w.shape[-1], np.float32)
+    ok = np.isfinite(m) & (m > 0)
+    _, e = np.frexp(np.where(ok, m, 1.0).astype(np.float32))        # m = f * 2^e, f in [0.5, 1)
+    return np.where(ok, np.ldexp(np.float32(1.0), e - 1), 1.0).astype(np.float32)
+
+
 class ConvPlan:
     """frcnn_conv_plan bound to fixed input/output/residual buffers (TMA descriptors hold raw pointers).
 
