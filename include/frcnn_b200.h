@@ -232,12 +232,12 @@ int frcnn_cls_finish(const float* head_out_dev, int ld, int r, int num_classes, 
                      const float* means4, float* cls_score_dev, float* cls_prob_dev, float* bbox_pred_dev,
                      void* stream);
 /* im_detect tail: boxes = rois[:,1:5]/scale; bbox_transform_inv; one-sided clip to the ORIGINAL image
- * (lib/model/test.py:95-102,67-77).  im_meta_dev [batch,3] fp32 = (im_scale, orig_h, orig_w) per image, read on the
+ * (lib/model/test.py:95-102,67-77).  r * num_classes must fit in int (else FRCNN_ERR_ARG).  im_meta_dev [batch,3] fp32 = (im_scale, orig_h, orig_w) per image, read on the
  * device (the launch is CUDA-graph capturable: the host only rewrites the 12 bytes).  pred_boxes_dev [r,4C] */
 int frcnn_bbox_decode(const float* rois_dev, const float* bbox_pred_dev, int r, int num_classes, int batch,
                       const float* im_meta_dev, float* pred_boxes_dev, void* stream);
 /* test_net tail (lib/model/test.py:162-180), per image: per class j>=1: score > thresh, NMS(flags, nms_thresh), then the
- * max_per_image cap over all classes.  r = RoI rows per image (<= 8192; above 1024 -- TEST.MODE='top' with
+ * max_per_image cap over all classes.  2 <= C <= 4096 classes (background included).  r = RoI rows per image (<= 8192; above 1024 -- TEST.MODE='top' with
  * RPN_TOP_N=5000 -- the kept sets live in `workspace_dev`, frcnn_detect_post_workspace_bytes(r, C, batch) bytes, else the
  * workspace may be NULL).  num_rois_dev: int32[batch] valid-row counts.  det_dev [batch,max_det,6] =
  * (x1,y1,x2,y2,score,class) sorted by (class, descending score); ndet_dev int32[batch] = the number of detections of
@@ -342,7 +342,7 @@ int frcnn_detect_post_soft_vote(const float* cls_prob_dev, const float* pred_box
  * row k of that image (classes ascending, slot = prefix(keep_cnt)[c] + j, slot < max_det).  fc7_dev [batch*r, feat_dim] is the
  * head output the class / box FC read (feat_dim % 4 == 0, 16-byte aligned).  roi_out_dev int32 [batch, max_det] = RoI index
  * within the image, -1 past the image's detection count; feat_out_dev [batch, max_det, feat_dim] = fc7 row of that RoI, zeros
- * past the count. */
+ * past the count.  2 <= C <= 4096 and r * C must fit in int (else FRCNN_ERR_ARG). */
 int frcnn_detect_features(const int* keep_dev, const int* keep_cnt_dev, const float* fc7_dev, int r, int batch, int num_classes,
                           int feat_dim, int max_det, float* feat_out_dev, int* roi_out_dev, void* stream);
 /* Bottom-up regions (Anderson et al. 2018, the protocol of bottom-up-attention's generate_tsv.py), an extension beyond the
@@ -360,15 +360,27 @@ int frcnn_detect_features(const int* keep_dev, const int* keep_cnt_dev, const fl
  *      descending conf_i, ties to the lower row.
  *   5. Region k of image b: boxes_out[b, k] = box_i, conf_out[b, k] = conf_i, class_out[b, k] = class_i, index_out[b, k] = i,
  *      feat_out[b, k] = fc7 row i; count_out[b] = the number of regions.  Rows k >= count_out[b] are zeros with index -1.
- * cls_prob entries must be >= +0 (softmax outputs).  Requirements: 2 <= C <= 1024, r <= 8192, conf_thresh in [0, 1],
- * 0 <= min_boxes <= max_boxes, max_boxes >= 1, feat_dim % 4 == 0.  Buffers (M = min(max_boxes, r)):
+ * cls_prob entries must be >= +0 (softmax outputs).  Requirements: 2 <= C <= 4096, r <= 8192, r * batch fits in int,
+ * conf_thresh in [0, 1], 0 <= min_boxes <= max_boxes, max_boxes >= 1, feat_dim % 4 == 0.
+ * Two implementations of step 2, chosen by C; both give the definition's result bit for bit:
+ *   C <= 1024: per-class NMS kernels (the post stage's) over the boxes broadcast to every class, then a fold of the kept lists;
+ *   C >  1024: one overlap bitmask per image (bit j of row i: does box_i suppress box_j; r * ceil(r/32) 32-bit words), then one greedy
+ *              walk of that mask per (class, image) in the class's score order.
+ * Buffers (M = min(max_boxes, r)):
  *   inputs  cls_prob_dev [batch*r, C], rois_dev [batch*r, 5], num_rois_dev int32 [batch], im_meta_dev [batch, 3] (as for
  *           frcnn_bbox_decode), fc7_dev [batch*r, feat_dim] (16-byte aligned);
- *   scratch keep_dev / keep_cnt_dev / keep_score_dev and workspace_dev as for frcnn_detect_post (they receive the per-class NMS of
- *           step 2, uncapped); roi_box_dev [batch*r, C, 4] fp32 (16-byte aligned); key_dev uint64 [batch*r] (8-byte aligned);
+ *   scratch C <= 1024: keep_dev / keep_cnt_dev / keep_score_dev and workspace_dev as for frcnn_detect_post (they receive the
+ *             per-class NMS of step 2, uncapped); roi_box_dev [batch*r, C, 4] fp32;
+ *           C > 1024: keep_dev / keep_cnt_dev / keep_score_dev are not used and may be NULL; workspace_dev (4-byte aligned) holds the
+ *             masks, batch * r * ceil(r/32) * 4 bytes; roi_box_dev [batch*r, 4] fp32;
+ *           both: workspace_bytes >= the frcnn_detect_regions_workspace_bytes of (r, C, batch) (at C <= 1024 that is
+ *             frcnn_detect_post_workspace_bytes, and the workspace may be NULL when r <= 1024); roi_box_dev 16-byte aligned;
+ *             key_dev uint64 [batch*r] (8-byte aligned);
  *   outputs boxes_out_dev [batch, M, 4] (16-byte aligned), conf_out_dev [batch, M], class_out_dev int32 [batch, M], index_out_dev
  *           int32 [batch, M], feat_out_dev [batch, M, feat_dim] (16-byte aligned), count_out_dev int32 [batch].
  * No allocation or synchronisation: capturable into a CUDA graph. */
+/* *bytes = the workspace frcnn_detect_regions needs for (r, C, batch); FRCNN_ERR_ARG outside its requirements */
+int frcnn_detect_regions_workspace_bytes(int r, int num_classes, int batch, size_t* bytes);
 int frcnn_detect_regions(const float* cls_prob_dev, const float* rois_dev, const int* num_rois_dev, const float* im_meta_dev,
                          const float* fc7_dev, int r, int batch, int num_classes, int feat_dim, float nms_thresh, unsigned flags,
                          float conf_thresh, int min_boxes, int max_boxes, int* keep_dev, int* keep_cnt_dev, float* keep_score_dev,

@@ -71,6 +71,7 @@ SIGNATURES = {
     "frcnn_cls_finish": (ci, [vp, ci, ci, ci, fp, fp, vp, vp, vp, vp]),
     "frcnn_bbox_decode": (ci, [vp, vp, ci, ci, ci, vp, vp, vp]),
     "frcnn_detect_post_workspace_bytes": (sz, [ci, ci, ci]),
+    "frcnn_detect_regions_workspace_bytes": (ci, [ci, ci, ci, C.POINTER(sz)]),
     "frcnn_detect_post": (ci, [vp, vp, vp, ci, ci, ci, cf, cf, cu, ci, ci, vp, vp, ci, vp, vp, vp, vp, sz, vp]),
     "frcnn_soft_nms_host": (ci, [fp, ip, ip, fp, ci, ci, ci, cf, cf, cf, ci]),
     "frcnn_detect_post_soft": (ci, [vp, vp, vp, ci, ci, ci, cf, ci, cf, cf, cf, ci, ci, vp, vp, ci, vp, vp, vp, vp, sz, vp]),

@@ -13,6 +13,7 @@
 // IoU arithmetic is the oracle's op-by-op fp32 sequence (__f*_rn: no FMA contraction) for all three predicate
 // variants (flags), so survivor indices are bit-exact.
 #include <cfloat>
+#include <climits>
 
 #include "common.cuh"
 #include "../../include/frcnn_b200.h"
@@ -333,6 +334,10 @@ __device__ __forceinline__ int count_ge(const float* __restrict__ sorted_desc, i
 }
 
 // VOTED: the record box of keep entry (c, j) is vote_box[img][c][j] (box voting) instead of pred[keep[c][j]].
+// Thread t holds the classes t, t + 1024, ... (CLS_PER_THREAD of them: C <= MAX_CLASSES); at C <= 1024 that is one class each.
+constexpr int MAX_CLASSES = 4096;
+constexpr int CLS_PER_THREAD = MAX_CLASSES / NMS_THREADS;
+
 template <bool VOTED>
 __global__ void __launch_bounds__(NMS_THREADS, 1)
 cap_emit_kernel(const float4* __restrict__ pred, int r, int C, int max_per_image, int max_det, int* __restrict__ keep,
@@ -340,14 +345,25 @@ cap_emit_kernel(const float4* __restrict__ pred, int r, int C, int max_per_image
                 int det_stride, int ndet_stride, const float4* __restrict__ vote_box) {
   __shared__ int s_warp[NMS_THREADS / 32];
   __shared__ int s_total;
-  __shared__ int s_off[1025];
+  __shared__ int s_off[MAX_CLASSES + 1];
   const int img = blockIdx.x;                       // one CTA per image of the batch
   pred += (size_t)img * r * C; keep += (size_t)img * C * r; keep_cnt += (size_t)img * C; keep_score += (size_t)img * C * r;
   det += (size_t)img * det_stride; ndet += (size_t)img * ndet_stride;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const bool is_cls = tid >= 1 && tid < C;
-  const int my_cnt = is_cls ? keep_cnt[tid] : 0;
-  const float* my_scores = keep_score + (size_t)tid * r;
+  int my_cnt[CLS_PER_THREAD], new_cnt[CLS_PER_THREAD];
+#pragma unroll
+  for (int q = 0; q < CLS_PER_THREAD; ++q) {
+    const int c = tid + q * NMS_THREADS;
+    my_cnt[q] = (c >= 1 && c < C) ? keep_cnt[c] : 0;
+    new_cnt[q] = my_cnt[q];
+  }
+  auto count_mine = [&](unsigned tbits) -> int {
+    int n = 0;
+#pragma unroll
+    for (int q = 0; q < CLS_PER_THREAD; ++q)
+      if (my_cnt[q]) n += count_ge(keep_score + (size_t)(tid + q * NMS_THREADS) * r, my_cnt[q], tbits);
+    return n;
+  };
   auto block_sum = [&](int v) -> int {
     for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     __syncthreads();
@@ -357,45 +373,60 @@ cap_emit_kernel(const float4* __restrict__ pred, int r, int C, int max_per_image
     __syncthreads();
     return s_total;
   };
-  const int total = block_sum(my_cnt);
-  int new_cnt = my_cnt;
+  int mine = 0;
+#pragma unroll
+  for (int q = 0; q < CLS_PER_THREAD; ++q) mine += my_cnt[q];
+  const int total = block_sum(mine);
   if (max_per_image > 0 && total > max_per_image) {
     unsigned t = 0u;                                   // largest pattern with count(score >= t) >= max_per_image
     for (int bit = 31; bit >= 0; --bit) {
       const unsigned cand = t | (1u << bit);
-      const int cnt = block_sum(is_cls ? count_ge(my_scores, my_cnt, cand) : 0);
+      const int cnt = block_sum(count_mine(cand));
       if (cnt >= max_per_image) t = cand;
     }
-    if (is_cls) new_cnt = count_ge(my_scores, my_cnt, t);
+#pragma unroll
+    for (int q = 0; q < CLS_PER_THREAD; ++q)
+      if (my_cnt[q]) new_cnt[q] = count_ge(keep_score + (size_t)(tid + q * NMS_THREADS) * r, my_cnt[q], t);
   }
-  if (is_cls) {
-    for (int j = new_cnt; j < my_cnt; ++j) keep[(size_t)tid * r + j] = -1;
-    keep_cnt[tid] = new_cnt;
-  }
-  // exclusive prefix of the per-class counts (C <= 1024: one thread per class, warp scan + warp totals)
-  int v = is_cls ? new_cnt : 0, incl = v;
-  for (int o = 1; o < 32; o <<= 1) { const int n = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += n; }
-  __syncthreads();
-  if (lane == 31) s_warp[warp] = incl;
-  __syncthreads();
-  int before = 0;
-  for (int w = 0; w < warp; ++w) before += s_warp[w];
-  if (tid <= C) s_off[tid] = before + incl - v;
-  if (tid == NMS_THREADS - 1) *ndet = before + incl;   // the TRUE count: the host rejects a record set that did not fit (> max_det)
-  __syncthreads();
-  for (int i = tid; i < (C - 1) * r; i += blockDim.x) {
-    const int c = 1 + i / r, j = i % r;
-    if (j < keep_cnt[c]) {
-      const int slot = s_off[c] + j;
-      if (slot < max_det) {
-        float4 b;
-        if (VOTED) b = __ldg(vote_box + ((size_t)img * C + c) * r + j);
-        else b = __ldg(pred + (size_t)keep[(size_t)c * r + j] * C + c);
-        float* d = det + (size_t)slot * 6;
-        d[0] = b.x; d[1] = b.y; d[2] = b.z; d[3] = b.w;
-        d[4] = keep_score[(size_t)c * r + j]; d[5] = (float)c;
-      }
+#pragma unroll
+  for (int q = 0; q < CLS_PER_THREAD; ++q) {
+    const int c = tid + q * NMS_THREADS;
+    if (c >= 1 && c < C) {
+      for (int j = new_cnt[q]; j < my_cnt[q]; ++j) keep[(size_t)c * r + j] = -1;
+      keep_cnt[c] = new_cnt[q];
     }
+  }
+  // exclusive prefix of the per-class counts in passes of 1024 classes (warp scan + warp totals), carried across passes
+  int carry = 0;
+  for (int base = 0; base < C; base += NMS_THREADS) {
+    const int c = base + tid, q = base / NMS_THREADS;
+    int v = 0;
+#pragma unroll
+    for (int k = 0; k < CLS_PER_THREAD; ++k) if (k == q && c >= 1 && c < C) v = new_cnt[k];
+    int incl = v;
+    for (int o = 1; o < 32; o <<= 1) { const int n = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += n; }
+    __syncthreads();
+    if (lane == 31) s_warp[warp] = incl;
+    __syncthreads();
+    int before = carry, pass = 0;
+    for (int w = 0; w < NMS_THREADS / 32; ++w) { const int s = s_warp[w]; before += w < warp ? s : 0; pass += s; }
+    if (c < C) s_off[c] = before + incl - v;
+    carry += pass;
+  }
+  if (tid == 0) { s_off[C] = carry; *ndet = carry; }   // the TRUE count: the host rejects a record set that did not fit (> max_det)
+  __syncthreads();
+  // records driven by slot: the class of a slot is the last c with s_off[c] <= slot
+  const int n = min(carry, max_det);
+  for (int slot = tid; slot < n; slot += blockDim.x) {
+    int lo = 1, hi = C;
+    while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (s_off[mid] <= slot) lo = mid; else hi = mid; }
+    const int c = lo, j = slot - s_off[c];
+    float4 b;
+    if (VOTED) b = __ldg(vote_box + ((size_t)img * C + c) * r + j);
+    else b = __ldg(pred + (size_t)keep[(size_t)c * r + j] * C + c);
+    float* d = det + (size_t)slot * 6;
+    d[0] = b.x; d[1] = b.y; d[2] = b.z; d[3] = b.w;
+    d[4] = keep_score[(size_t)c * r + j]; d[5] = (float)c;
   }
 }
 
@@ -795,39 +826,45 @@ box_vote_set_kernel(const float* __restrict__ top, int n_top, int top_dim, const
 // ---- per-detection head features ---------------------------------------------------------------------------
 // Runs after cap_emit_kernel and rebuilds its slot order from the truncated keep lists (classes ascending, slot =
 // prefix(keep_cnt)[c] + j), so slot k of the features is record row k.  One CTA per (block of FEAT_SLOTS slots, image):
-// each thread scans 4 consecutive class counts (C <= 1024), then the CTA copies its slots' fc7 rows, float4 wide.
+// each thread scans 4 consecutive class counts per pass of 1024 classes (C <= MAX_CLASSES), then the CTA copies its slots' fc7 rows,
+// float4 wide.
 constexpr int FEAT_THREADS = 256;
 constexpr int FEAT_SLOTS = 8;
 
 __global__ void __launch_bounds__(FEAT_THREADS)
 detect_features_kernel(const int* __restrict__ keep, const int* __restrict__ keep_cnt, const float4* __restrict__ fc7, int r, int C,
                        int f4, int max_det, float4* __restrict__ feat_out, int* __restrict__ roi_out) {
-  __shared__ int s_off[1025];
+  __shared__ int s_off[MAX_CLASSES + 1];
   __shared__ int s_warp[FEAT_THREADS / 32];
   __shared__ int s_roi[FEAT_SLOTS];
   const int img = blockIdx.y, slot0 = blockIdx.x * FEAT_SLOTS;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   keep += (size_t)img * C * r; keep_cnt += (size_t)img * C;
-  int cnt[4], v = 0;
+  int carry = 0;                                                // passes of 4 * FEAT_THREADS classes, carried
+  for (int base = 0; base < C; base += 4 * FEAT_THREADS) {
+    int cnt[4], v = 0;
 #pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    const int c = 4 * tid + q;
-    cnt[q] = (c >= 1 && c < C) ? __ldg(keep_cnt + c) : 0;     // class 0 (background) never emits
-    v += cnt[q];
-  }
-  int incl = v;
-  for (int o = 1; o < 32; o <<= 1) { const int n = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += n; }
-  if (lane == 31) s_warp[warp] = incl;
-  __syncthreads();
-  int run = incl - v;
-  for (int w = 0; w < warp; ++w) run += s_warp[w];
+    for (int q = 0; q < 4; ++q) {
+      const int c = base + 4 * tid + q;
+      cnt[q] = (c >= 1 && c < C) ? __ldg(keep_cnt + c) : 0;   // class 0 (background) never emits
+      v += cnt[q];
+    }
+    int incl = v;
+    for (int o = 1; o < 32; o <<= 1) { const int n = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += n; }
+    if (base) __syncthreads();                                  // the previous pass has read s_warp
+    if (lane == 31) s_warp[warp] = incl;
+    __syncthreads();
+    int run = carry + incl - v;
+    for (int w = 0; w < warp; ++w) run += s_warp[w];
 #pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    const int c = 4 * tid + q;
-    if (c < C) s_off[c] = run;
-    run += cnt[q];
+    for (int q = 0; q < 4; ++q) {
+      const int c = base + 4 * tid + q;
+      if (c < C) s_off[c] = run;
+      run += cnt[q];
+    }
+    for (int w = 0; w < FEAT_THREADS / 32; ++w) carry += s_warp[w];
   }
-  if (tid == FEAT_THREADS - 1) s_off[C] = run;                  // detections of the image (the record's ndet)
+  if (tid == 0) s_off[C] = carry;                               // detections of the image (the record's ndet)
   __syncthreads();
   if (tid < FEAT_SLOTS) {
     const int slot = slot0 + tid;
@@ -885,10 +922,10 @@ __global__ void regions_fold_kernel(const int* __restrict__ keep, const int* __r
 
 // one CTA per image: count conf >= thresh, then either the ascending compaction (min_boxes <= count <= max_boxes) or a bitonic sort
 // of the cap (conf, ~index) keys, descending (conf descending, ties to the lower index); then the outputs of rows [0, max_out).
-// Dynamic shared memory: cap (power of two >= r) 64-bit words.
+// Dynamic shared memory: cap (power of two >= r) 64-bit words.  box_stride: float4 boxes per RoI row of roi_box (C or 1).
 __global__ void __launch_bounds__(REGION_THREADS, 1)
 regions_select_kernel(const unsigned long long* __restrict__ key, const float4* __restrict__ roi_box, const int* __restrict__ num_rois,
-                      int r, int C, int cap, float conf_thresh, int min_boxes, int max_boxes, int max_out, float* __restrict__ boxes_out,
+                      int r, int box_stride, int cap, float conf_thresh, int min_boxes, int max_boxes, int max_out, float* __restrict__ boxes_out,
                       float* __restrict__ conf_out, int* __restrict__ class_out, int* __restrict__ index_out, int* __restrict__ count_out) {
   extern __shared__ __align__(16) unsigned long long sel[];
   __shared__ int s_warp[REGION_THREADS / 32];
@@ -950,13 +987,127 @@ regions_select_kernel(const unsigned long long* __restrict__ key, const float4* 
       const unsigned cb = (unsigned)(kk >> 32);
       cf = __uint_as_float(cb);
       cl = cb ? (int)~(unsigned)kk : 0;
-      b = roi_box[((size_t)img * r + i) * C];
+      b = roi_box[((size_t)img * r + i) * box_stride];
     }
     const size_t o = (size_t)img * max_out + k;
     reinterpret_cast<float4*>(boxes_out)[o] = b;
     conf_out[o] = cf; class_out[o] = cl; index_out[o] = i;
   }
   if (tid == 0) count_out[img] = n;
+}
+
+// ---- bottom-up regions above REGIONS_CLASS_NMS_MAX classes: one overlap mask per image, one greedy walk per (class, image) ----------
+// Every class runs greedy NMS over the same unregressed boxes, so the overlaps are computed once per image: mask[img][i][w] bit b =
+// suppresses(box_i, box_{32w+b}) with the canonical boxes and areas class_nms_kernel uses (suppresses is symmetric in its two
+// boxes), rows and columns >= nr empty.  A class then only needs its score order and a walk over the mask: the next row in order that
+// no kept row has removed is kept, and removes its mask row.  That is block_greedy_nms's result, row for row.
+constexpr int REGIONS_CLASS_NMS_MAX = 1024;   // frcnn_detect_regions: per-class NMS + fold up to this C, the mask walk above
+constexpr int WALK_WARPS = 8;                 // r <= DET_CAP: one warp per class, 8 classes per CTA sharing the image's mask
+
+__host__ __device__ constexpr int mask_words(int r) { return (r + 31) / 32; }
+
+// thread per mask word (row i, word w) of image blockIdx.y; box [batch*r] float4 (regions_boxes_kernel with C = 1)
+__global__ void regions_mask_kernel(const float4* __restrict__ box, const int* __restrict__ num_rois, int r, float thr, unsigned flags,
+                                    unsigned* __restrict__ mask) {
+  const int img = blockIdx.y, W = mask_words(r);
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;         // r * W <= 8192 * 256
+  if (e >= r * W) return;
+  const int i = e / W, w = e - i * W;
+  const int nr = min(__ldg(num_rois + img), r);
+  box += (size_t)img * r;
+  unsigned bits = 0u;
+  if (i < nr && thr >= 0.f) {                                   // thr < 0: block_greedy_nms suppresses nothing
+    const float4 a = canon(__ldg(box + i), flags);
+    const float aa = box_area(a, flags);
+    const int nb = min(32, nr - w * 32);
+    for (int b = 0; b < nb; ++b) {
+      const float4 o = canon(__ldg(box + w * 32 + b), flags);
+      if (suppresses(a, aa, o, box_area(o, flags), thr, flags)) bits |= 1u << b;
+    }
+  }
+  mask[((size_t)img * r + i) * W + w] = bits;
+}
+
+// One unit per (foreground class, image).  BIG = false (r <= DET_CAP): a warp per unit, WALK_WARPS units per CTA; the CTA copies the
+// image's mask rows into shared memory, each warp sorts its class in its own cap slots.  BIG = true (r <= DET_CAP_BIG): a CTA of
+// NMS_THREADS per unit sorts, warp 0 walks with the mask rows read from global memory.  The sort is class_nms_kernel's (candidates
+// score > -1, i.e. every valid row; key desc, row asc; the rest -inf at the tail).  The removed set is one register word per lane
+// (!BIG) or mask_words(r) words of shared memory (BIG).  Each kept row is folded into the per-RoI key as regions_fold_kernel does.
+// Dynamic shared memory: BIG: cap floats | cap ints | mask_words(r) words;  !BIG: mask_words(r) * r words (rounded to 4) | WALK_WARPS x (cap floats | cap ints).
+template <bool BIG>
+__global__ void __launch_bounds__(BIG ? NMS_THREADS : WALK_WARPS * 32)
+regions_walk_kernel(const float* __restrict__ probs, const unsigned* __restrict__ mask, const int* __restrict__ num_rois, int r, int C,
+                    int cap, unsigned long long* __restrict__ key) {
+  extern __shared__ __align__(16) unsigned walk_dyn[];
+  const int img = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, W = mask_words(r);
+  const int nr = min(__ldg(num_rois + img), r);
+  mask += (size_t)img * r * W;
+  const unsigned* rows = mask;
+  float* skey;
+  int cls, g, G;                                                // this thread is g of the G sorting the class
+  if (BIG) {
+    skey = reinterpret_cast<float*>(walk_dyn);
+    cls = blockIdx.x + 1; g = tid; G = NMS_THREADS;
+  } else {
+    for (int k = tid; k < nr * W; k += blockDim.x) walk_dyn[k] = __ldg(mask + k);
+    rows = walk_dyn;
+    skey = reinterpret_cast<float*>(walk_dyn + ((r * W + 3) & ~3)) + (size_t)warp * 2 * cap;
+    cls = blockIdx.x * WALK_WARPS + warp + 1; g = lane; G = 32;
+    __syncthreads();
+    if (cls >= C) return;
+  }
+  int* sidx = reinterpret_cast<int*>(skey + cap);
+  auto sync = [&] { if (BIG) __syncthreads(); else __syncwarp(); };
+  probs += (size_t)img * r * C;
+  for (int e = g; e < cap; e += G) {
+    float k = __int_as_float(0xff800000);
+    if (e < nr) {
+      const float s = __ldg(probs + (size_t)e * C + cls);
+      if (s > -1.f) k = s;
+    }
+    skey[e] = k; sidx[e] = e;
+  }
+  for (int k = 2; k <= cap; k <<= 1) {
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      sync();
+      for (int e = g; e < cap; e += G) {
+        const int ixj = e ^ j;
+        if (ixj > e) {
+          const float a = skey[e], b = skey[ixj];
+          const int ia = sidx[e], ib = sidx[ixj];
+          const bool a_first = (a > b) || (a == b && ia < ib);
+          const bool up = (e & k) == 0;
+          if (up ? !a_first : a_first) { skey[e] = b; skey[ixj] = a; sidx[e] = ib; sidx[ixj] = ia; }
+        }
+      }
+    }
+  }
+  sync();
+  if (BIG && warp != 0) return;
+  unsigned rem = 0u;                                            // !BIG: word `lane` of the removed set
+  unsigned* srem = reinterpret_cast<unsigned*>(sidx + cap);     // BIG: the removed set in shared memory
+  if (BIG) {
+    for (int k = lane; k < W; k += 32) srem[k] = 0u;
+    __syncwarp();
+  }
+  const unsigned long long low = (unsigned)~cls;
+  unsigned long long* krow = key + (size_t)img * r;
+  for (int p = 0; p < cap; ++p) {
+    const float s = skey[p];
+    if (!(s > -1.f)) break;                                     // the -inf tail: no candidates left
+    const int row = sidx[p];
+    const unsigned wv = BIG ? srem[row >> 5] : __shfl_sync(0xffffffffu, rem, row >> 5);
+    if ((wv >> (row & 31)) & 1u) continue;                      // removed by a kept row
+    if (lane == 0) atomicMax(krow + row, ((unsigned long long)__float_as_uint(s) << 32) | low);
+    const unsigned* m = rows + (size_t)row * W;
+    if (BIG) {
+      __syncwarp();                                             // every lane has read srem
+      for (int k = lane; k < W; k += 32) srem[k] |= __ldg(m + k);
+      __syncwarp();
+    } else if (lane < W) {
+      rem |= m[lane];
+    }
+  }
 }
 
 // one CTA per (block of FEAT_SLOTS output rows, image): fc7 row of each selected RoI, zeros past the count
@@ -1060,6 +1211,14 @@ extern "C" size_t frcnn_detect_post_workspace_bytes(int r, int num_classes, int 
   return (size_t)batch * num_classes * (size_t)((r + 3) & ~3) * 24 + 256;
 }
 
+extern "C" int frcnn_detect_regions_workspace_bytes(int r, int num_classes, int batch, size_t* bytes) {
+  FRCNN_REQUIRE(bytes && r > 0 && batch > 0 && num_classes >= 2 && num_classes <= MAX_CLASSES,
+                "detect_regions_workspace_bytes: bytes != NULL, r>0, batch>0, 2<=C<=%d required", MAX_CLASSES);
+  *bytes = num_classes <= REGIONS_CLASS_NMS_MAX ? frcnn_detect_post_workspace_bytes(r, num_classes, batch)
+                                                : (size_t)batch * r * mask_words(r) * 4 + 256;
+  return OK;
+}
+
 static int soft_params(int method, float sigma, float nt, float score_thresh, SoftParams* p, const char* who) {
   FRCNN_REQUIRE(method == FRCNN_SOFT_NMS_LINEAR || method == FRCNN_SOFT_NMS_GAUSSIAN || method == FRCNN_SOFT_NMS_HARD,
                 "%s: method %d is not FRCNN_SOFT_NMS_LINEAR / _GAUSSIAN / _HARD", who, method);
@@ -1101,9 +1260,10 @@ static int detect_post_run(const char* who, const float* cls_prob, const float* 
                            int* keep, int* keep_cnt, float* keep_score, const VoteParams* vote, float* vote_box, void* stream,
                            ClassStage class_stage) {
   FRCNN_REQUIRE(cls_prob && pred_boxes && num_rois && det && ndet && keep && keep_cnt && keep_score, "%s: null pointer", who);
-  FRCNN_REQUIRE(r > 0 && batch > 0 && num_classes >= 2 && num_classes <= 1024, "%s: r>0, batch>0, 2<=C<=1024 required", who);
+  FRCNN_REQUIRE(r > 0 && batch > 0 && num_classes >= 2 && num_classes <= MAX_CLASSES, "%s: r>0, batch>0, 2<=C<=%d required", who,
+                MAX_CLASSES);
   if (r > DET_CAP_BIG) { set_error("%s: %d RoIs per image > capacity %d", who, r, DET_CAP_BIG); return ERR_CAPACITY; }
-  FRCNN_REQUIRE(record_stride == 0 || record_stride >= max_det * 6, "%s: record_stride %d < max_det*6", who, record_stride);
+  FRCNN_REQUIRE(record_stride == 0 || record_stride >= (long long)max_det * 6, "%s: record_stride %d < max_det*6", who, record_stride);
   FRCNN_REQUIRE(!vote || (vote_box && ((uintptr_t)vote_box & 15) == 0), "%s: vote_box must be a 16-byte aligned device buffer", who);
   cudaStream_t st = (cudaStream_t)stream;
   const float4* pred = reinterpret_cast<const float4*>(pred_boxes);
@@ -1318,8 +1478,9 @@ extern "C" int frcnn_soft_nms_host(float* dets_out, int* keep_out, int* num_out,
 extern "C" int frcnn_detect_features(const int* keep, const int* keep_cnt, const float* fc7, int r, int batch, int num_classes,
                                      int feat_dim, int max_det, float* feat_out, int* roi_out, void* stream) {
   FRCNN_REQUIRE(keep && keep_cnt && fc7 && feat_out && roi_out, "detect_features: null pointer");
-  FRCNN_REQUIRE(r > 0 && batch > 0 && num_classes >= 2 && num_classes <= 1024 && max_det > 0,
-                "detect_features: r>0, batch>0, 2<=C<=1024, max_det>0 required");
+  FRCNN_REQUIRE(r > 0 && batch > 0 && num_classes >= 2 && num_classes <= MAX_CLASSES && max_det > 0,
+                "detect_features: r>0, batch>0, 2<=C<=%d, max_det>0 required", MAX_CLASSES);
+  FRCNN_REQUIRE((long long)r * num_classes <= INT_MAX, "detect_features: r*C = %lld does not fit in int", (long long)r * num_classes);
   FRCNN_REQUIRE(feat_dim > 0 && feat_dim % 4 == 0 && ((uintptr_t)fc7 & 15) == 0 && ((uintptr_t)feat_out & 15) == 0,
                 "detect_features: feat_dim %d must be a positive multiple of 4 and fc7 / feat_out 16-byte aligned", feat_dim);
   const dim3 grid((unsigned)cdiv(max_det, FEAT_SLOTS), (unsigned)batch);
@@ -1335,35 +1496,66 @@ extern "C" int frcnn_detect_regions(const float* cls_prob, const float* rois, co
                                     int min_boxes, int max_boxes, int* keep, int* keep_cnt, float* keep_score, void* workspace,
                                     size_t workspace_bytes, float* roi_box, unsigned long long* key, float* boxes_out, float* conf_out,
                                     int* class_out, int* index_out, float* feat_out, int* count_out, void* stream) {
-  FRCNN_REQUIRE(cls_prob && rois && num_rois && im_meta && fc7 && keep && keep_cnt && keep_score && roi_box && key && boxes_out &&
-                conf_out && class_out && index_out && feat_out && count_out, "detect_regions: null pointer");
-  FRCNN_REQUIRE(r > 0 && batch > 0 && num_classes >= 2 && num_classes <= 1024, "detect_regions: r>0, batch>0, 2<=C<=1024 required");
+  const bool walk = num_classes > REGIONS_CLASS_NMS_MAX;        // the overlap-mask path: keep / keep_cnt / keep_score are not used
+  FRCNN_REQUIRE(cls_prob && rois && num_rois && im_meta && fc7 && (walk || (keep && keep_cnt && keep_score)) && roi_box && key &&
+                boxes_out && conf_out && class_out && index_out && feat_out && count_out, "detect_regions: null pointer");
+  FRCNN_REQUIRE(r > 0 && batch > 0 && num_classes >= 2 && num_classes <= MAX_CLASSES, "detect_regions: r>0, batch>0, 2<=C<=%d required",
+                MAX_CLASSES);
   if (r > REGION_CAP) { set_error("detect_regions: %d RoIs per image > capacity %d", r, REGION_CAP); return ERR_CAPACITY; }
+  FRCNN_REQUIRE((long long)r * batch <= INT_MAX, "detect_regions: r*batch = %lld does not fit in int", (long long)r * batch);
   FRCNN_REQUIRE(feat_dim > 0 && feat_dim % 4 == 0 && ((uintptr_t)fc7 & 15) == 0 && ((uintptr_t)feat_out & 15) == 0,
                 "detect_regions: feat_dim %d must be a positive multiple of 4 and fc7 / feat_out 16-byte aligned", feat_dim);
   FRCNN_REQUIRE(((uintptr_t)roi_box & 15) == 0 && ((uintptr_t)boxes_out & 15) == 0 && ((uintptr_t)key & 7) == 0,
                 "detect_regions: roi_box / boxes_out must be 16-byte and key 8-byte aligned");
   FRCNN_REQUIRE(conf_thresh >= 0.f && conf_thresh <= 1.f, "detect_regions: conf_thresh must lie in [0, 1]");
   FRCNN_REQUIRE(min_boxes >= 0 && max_boxes >= 1 && min_boxes <= max_boxes, "detect_regions: 0 <= min_boxes <= max_boxes, max_boxes >= 1 required");
-  FRCNN_REQUIRE(r <= DET_CAP || (workspace && workspace_bytes >= frcnn_detect_post_workspace_bytes(r, num_classes, batch)),
-                "detect_regions: workspace too small");
+  size_t need = 0;
+  if (walk)
+    FRCNN_REQUIRE(workspace && ((uintptr_t)workspace & 3) == 0 && frcnn_detect_regions_workspace_bytes(r, num_classes, batch, &need) == OK &&
+                  workspace_bytes >= need, "detect_regions: workspace too small");
+  else
+    FRCNN_REQUIRE(r <= DET_CAP || (workspace && workspace_bytes >= frcnn_detect_post_workspace_bytes(r, num_classes, batch)),
+                  "detect_regions: workspace too small");
   cudaStream_t st = (cudaStream_t)stream;
   float4* rb = reinterpret_cast<float4*>(roi_box);
   const int rows = r * batch;
-  regions_boxes_kernel<<<(unsigned)(((size_t)rows * num_classes + 255) / 256), 256, 0, st>>>(rois, im_meta, r, num_classes, rows, rb, key);
-  FRCNN_LAUNCH_CHECK();
-  // every valid row is a candidate of every class: score_thresh -1 < any score >= +0
-  if (int rc = class_nms_launch(dim3((unsigned)(num_classes - 1), (unsigned)batch), st, cls_prob, rb, num_rois, r, batch, num_classes, -1.f,
-                                nms_thresh, flags, keep, keep_cnt, keep_score, workspace, workspace_bytes)) return rc;
-  FRCNN_LAUNCH_CHECK();
-  regions_fold_kernel<<<dim3((unsigned)(num_classes - 1), (unsigned)batch), 256, 0, st>>>(keep, keep_cnt, keep_score, r, num_classes, key);
-  FRCNN_LAUNCH_CHECK();
-  int cap = 1;
+  const int box_stride = walk ? 1 : num_classes;
+  int cap = 1;                                                  // sort capacity: power of two >= r
   while (cap < r) cap <<= 1;
+  regions_boxes_kernel<<<(unsigned)(((size_t)rows * box_stride + 255) / 256), 256, 0, st>>>(rois, im_meta, r, box_stride, rows, rb, key);
+  FRCNN_LAUNCH_CHECK();
+  if (walk) {
+    unsigned* mask = reinterpret_cast<unsigned*>(workspace);
+    const int W = mask_words(r);
+    regions_mask_kernel<<<dim3((unsigned)cdiv(r * W, 256), (unsigned)batch), 256, 0, st>>>(rb, num_rois, r, nms_thresh, flags, mask);
+    FRCNN_LAUNCH_CHECK();
+    if (r <= DET_CAP) {
+      static bool attr_done[MAX_DEVICES];
+      const size_t smem_max = (size_t)DET_CAP * mask_words(DET_CAP) * 4 + (size_t)WALK_WARPS * DET_CAP * 8;
+      if (int rc = smem_attr_once(regions_walk_kernel<false>, smem_max, attr_done)) return rc;
+      const size_t smem = (size_t)((r * W + 3) & ~3) * 4 + (size_t)WALK_WARPS * cap * 8;
+      regions_walk_kernel<false><<<dim3((unsigned)cdiv(num_classes - 1, WALK_WARPS), (unsigned)batch), WALK_WARPS * 32, smem, st>>>(
+          cls_prob, mask, num_rois, r, num_classes, cap, key);
+    } else {
+      static bool attr_done[MAX_DEVICES];
+      const size_t smem_max = (size_t)DET_CAP_BIG * 8 + (size_t)mask_words(DET_CAP_BIG) * 4;
+      if (int rc = smem_attr_once(regions_walk_kernel<true>, smem_max, attr_done)) return rc;
+      regions_walk_kernel<true><<<dim3((unsigned)(num_classes - 1), (unsigned)batch), NMS_THREADS, (size_t)cap * 8 + (size_t)W * 4, st>>>(
+          cls_prob, mask, num_rois, r, num_classes, cap, key);
+    }
+    FRCNN_LAUNCH_CHECK();
+  } else {
+    // every valid row is a candidate of every class: score_thresh -1 < any score >= +0
+    if (int rc = class_nms_launch(dim3((unsigned)(num_classes - 1), (unsigned)batch), st, cls_prob, rb, num_rois, r, batch, num_classes, -1.f,
+                                  nms_thresh, flags, keep, keep_cnt, keep_score, workspace, workspace_bytes)) return rc;
+    FRCNN_LAUNCH_CHECK();
+    regions_fold_kernel<<<dim3((unsigned)(num_classes - 1), (unsigned)batch), 256, 0, st>>>(keep, keep_cnt, keep_score, r, num_classes, key);
+    FRCNN_LAUNCH_CHECK();
+  }
   static bool attr_done[MAX_DEVICES];
   if (int rc = smem_attr_once(regions_select_kernel, (size_t)REGION_CAP * 8, attr_done)) return rc;
   const int max_out = max_boxes < r ? max_boxes : r;
-  regions_select_kernel<<<(unsigned)batch, REGION_THREADS, (size_t)cap * 8, st>>>(key, rb, num_rois, r, num_classes, cap, conf_thresh,
+  regions_select_kernel<<<(unsigned)batch, REGION_THREADS, (size_t)cap * 8, st>>>(key, rb, num_rois, r, box_stride, cap, conf_thresh,
                                                                                   min_boxes, max_boxes, max_out, boxes_out, conf_out,
                                                                                   class_out, index_out, count_out);
   FRCNN_LAUNCH_CHECK();

@@ -3,6 +3,7 @@
 // nvcc cannot contract them; reference file:line citations are in include/frcnn_b200.h.
 #include <cuda_fp16.h>
 #include <math.h>
+#include <climits>
 #include "common.cuh"
 #include "../../include/frcnn_b200.h"
 
@@ -772,6 +773,7 @@ extern "C" int frcnn_cls_finish(const float* head_out, int ld, int r, int num_cl
 extern "C" int frcnn_bbox_decode(const float* rois, const float* bbox_pred, int r, int num_classes, int batch, const float* im_meta_dev,
                                  float* pred_boxes, void* stream) {
   FRCNN_REQUIRE(rois && bbox_pred && pred_boxes && im_meta_dev && batch > 0, "bbox_decode: bad argument");
+  FRCNN_REQUIRE((long long)r * num_classes <= INT_MAX, "bbox_decode: r*C = %lld does not fit in int", (long long)r * num_classes);
   bbox_decode_kernel<<<blocks_for((long)r * num_classes, 256), 256, 0, (cudaStream_t)stream>>>(rois, bbox_pred, r, num_classes, batch,
                                                                                              im_meta_dev, pred_boxes);
   FRCNN_LAUNCH_CHECK();

@@ -250,7 +250,7 @@ class PostStage:
         self.net, self.batch = net, batch
         self.post_key = None
         self.regions_key = self.regions_step = None                 # region mode (_ensure_regions)
-        self.reg_box = self.reg_key = self.reg_out = None
+        self.reg_box = self.reg_key = self.reg_out = self.reg_ws = None
         self.recs = [None, None]
         self.rec = self.ndet = None    # views of the buffer the LAST detect launch wrote
         self.post_steps = [None, None]
@@ -309,16 +309,20 @@ class PostStage:
 
     def _ensure_regions(self, conf_thresh, min_boxes, max_boxes):
         """(Re)build the bottom-up regions step for region_args' (fp32 conf_thresh, min_boxes, max_boxes) and the NMS options in
-        force.  Its buffers are allocated on first use: the RoI boxes broadcast over the classes, the per-RoI keys and
-        min(max_boxes, R) output rows per image; the per-class NMS reuses keep / keep_cnt / keep_score / post_ws."""
+        force.  Its buffers are allocated on first use: the RoI boxes (broadcast over the classes up to
+        ops.REGIONS_CLASS_NMS_MAX classes, one per row above), the per-RoI keys and min(max_boxes, R) output rows per image.  Up to
+        REGIONS_CLASS_NMS_MAX classes the per-class NMS reuses keep / keep_cnt / keep_score / post_ws; above, the step needs only its
+        own workspace (the per-image overlap masks)."""
         o = self.net.options
         key = RegionKey(float(conf_thresh), int(min_boxes), int(max_boxes), float(o["nms_thresh"]), bool(o["use_gpu_nms"]))
         if key == self.regions_key:
             return
         C, R, B = self.net.num_classes, self.R, self.batch
+        per_class = C <= ops.REGIONS_CLASS_NMS_MAX
         if self.reg_box is None:
-            self.reg_box = ops.zeros((B * R, C, 4))
+            self.reg_box = ops.zeros(ops.regions_box_shape(B * R, C))
             self.reg_key = ops.zeros((B * R,), dtype=torch.int64)
+            self.reg_ws = self.post_ws if per_class else ops.detect_regions_workspace(R, C, B)
         M = min(key.max_boxes, R)
         if self.reg_out is None or self.reg_out["conf"].shape[1] != M:
             fdim = int(self.fc7.shape[1])
@@ -327,9 +331,10 @@ class PostStage:
                                 count=ops.zeros((B,), dtype=torch.int32))
         thr, flags = nms_threshold(key.nms_thresh, key.use_gpu_nms)
         out = self.reg_out
+        keep = (self.keep, self.keep_cnt, self.keep_score) if per_class else (None, None, None)
         self.regions_step = lambda: ops.detect_regions(self.cls_prob, self.rois, self.num_rois, self.im_meta, self.fc7, C, thr, flags,
-                                                       key.conf_thresh, key.min_boxes, key.max_boxes, self.keep, self.keep_cnt,
-                                                       self.keep_score, self.post_ws, self.reg_box, self.reg_key, out, batch=B)
+                                                       key.conf_thresh, key.min_boxes, key.max_boxes, *keep, self.reg_ws, self.reg_box,
+                                                       self.reg_key, out, batch=B)
         for g in [g for g in self.graphs if isinstance(g, tuple) and g[0] == "regions"]:
             del self.graphs[g]
         self.regions_key = key
@@ -533,7 +538,7 @@ class ShapePlan(PostStage):
         self.rec = self.ndet = None
         self.feat_out = self.roi_out = self.features_step = None
         self.regions_key = self.regions_step = None
-        self.reg_box = self.reg_key = self.reg_out = None
+        self.reg_box = self.reg_key = self.reg_out = self.reg_ws = None
 
     def steps_for(self, mode):
         """mode: 'test_image' (network outputs), 'im_detect' (+ decoded boxes), 'detect' (+ per-class NMS, cap, records),
@@ -793,6 +798,16 @@ def f32_not_below(t):
 
 def _is_int(v):
     return isinstance(v, (int, np.integer)) and not isinstance(v, (bool, np.bool_))
+
+
+MAX_CLASSES = 4096   # classes (background included) every detection path handles (include/frcnn_b200.h)
+
+
+def check_num_classes(num_classes):
+    """The class count of a network: an int in [2, MAX_CLASSES], else ValueError."""
+    if not _is_int(num_classes) or not 2 <= num_classes <= MAX_CLASSES:
+        raise ValueError("num_classes must be an integer in [2, %d] (background included), got %r" % (MAX_CLASSES, num_classes))
+    return int(num_classes)
 
 
 def region_args(conf_thresh, min_boxes, max_boxes):

@@ -38,6 +38,7 @@ class Network(object):
         assert tag is not None
         if mode != "TEST":
             raise NotImplementedError("only the TEST-mode (inference) graph exists in this build")
+        num_classes = engine.check_num_classes(num_classes)
         self._mode, self._tag = mode, tag
         self._num_classes = num_classes
         self._anchor_scales, self._anchor_ratios = tuple(anchor_scales), tuple(anchor_ratios)

@@ -325,11 +325,31 @@ def detect_features(keep, keep_cnt, fc7, num_classes, feat_out, roi_out):
                                           _p(roi_out), _stream()), "detect_features")
 
 
+# frcnn_detect_regions runs the per-class NMS up to this many classes and the per-image overlap mask above (include/frcnn_b200.h)
+REGIONS_CLASS_NMS_MAX = 1024
+
+
+def regions_box_shape(rows, num_classes):
+    """Shape of detect_regions' roi_box scratch: the RoI box broadcast to every class, or one box per row on the mask path."""
+    return (rows, num_classes, 4) if num_classes <= REGIONS_CLASS_NMS_MAX else (rows, 4)
+
+
+def detect_regions_workspace_bytes(r, num_classes, batch=1):
+    n = C.c_size_t(0)
+    N.check(N.lib().frcnn_detect_regions_workspace_bytes(r, num_classes, batch, C.byref(n)), "detect_regions_workspace_bytes")
+    return n.value
+
+
+def detect_regions_workspace(r, num_classes, batch=1):
+    return torch.empty(detect_regions_workspace_bytes(r, num_classes, batch), dtype=torch.uint8, device="cuda")
+
+
 def detect_regions(cls_prob, rois, num_rois, im_meta, fc7, num_classes, nms_thresh, flags, conf_thresh, min_boxes, max_boxes, keep,
                    keep_cnt, keep_score, workspace, roi_box, key, out, batch=1):
     """Bottom-up regions (frcnn_detect_regions): cls_prob [batch*r, C], rois [batch*r, 5], num_rois int32 [batch], im_meta
-    [batch, 3], fc7 [batch*r, F]; keep / keep_cnt / keep_score / workspace as for detect_post; roi_box [batch*r, C, 4] fp32 and
-    key int64 [batch*r] scratch.  out: dict of boxes [batch, M, 4], conf [batch, M], classes int32 [batch, M], roi_index int32
+    [batch, 3], fc7 [batch*r, F]; workspace of detect_regions_workspace(r, C, batch) bytes or more; keep / keep_cnt / keep_score
+    as for detect_post up to REGIONS_CLASS_NMS_MAX classes (unused, may be None, above); roi_box regions_box_shape(batch*r, C) fp32
+    and key int64 [batch*r] scratch.  out: dict of boxes [batch, M, 4], conf [batch, M], classes int32 [batch, M], roi_index int32
     [batch, M], features [batch, M, F], count int32 [batch] with M = min(max_boxes, r).  conf_thresh is the fp32 threshold."""
     r = cls_prob.shape[0] // batch
     fdim = fc7.shape[1]
