@@ -10,7 +10,7 @@ not only where its outputs reach the post:
   bit-equal with no tile and with every tile split, and on every tile the ragged split treats alike in both orders;
 * cls_finish at 1025 to 4096 classes (test_stage_edges_gpu's edge body: every logit row kind, NaN in the pad columns) and
   bbox_decode at 1025 to 4096 classes with three images, and at 5000 RoIs x 4096 classes;
-* the detect graph audited step by step (test_graph_audit_gpu's run_audit, unchanged) at 1204 to 4096 classes, with teeth: one
+* the detect graph audited step by step (graph_audit's run_audit, unchanged) at 1204 to 4096 classes, with teeth: one
   element of the head's last N tile moved by 1e-3 relative, and two cls_score columns swapped in the engine's weights, each
   fail at the cls_bbox layer;
 * Soft-NMS, box voting and the flip augmentation of a 1601-class ResNet-101 against the oracles' post of its own outputs.
@@ -39,7 +39,7 @@ import soft_nms_oracle as SO  # noqa: E402
 import stage_ref64 as S  # noqa: E402
 from oracle import pipeline as P  # noqa: E402
 from test_conv_gpu import ALPHA, BETA, conv_run, epilogue64, ratio, reference  # noqa: E402
-from test_graph_audit_gpu import build as audit_build, run_audit  # noqa: E402
+from graph_audit import build as audit_build, run_audit  # noqa: E402
 from test_regions_gpu import _release_networks, build as net_build  # noqa: E402,F401
 from test_soft_nms_gpu import own_outputs, records_from  # noqa: E402
 from test_stage_edges_gpu import check_decode_per_image, decode_rois, run_bbox_decode  # noqa: E402

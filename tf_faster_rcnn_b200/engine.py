@@ -757,6 +757,9 @@ def roi_align_option(pooling_mode, pooling_size, node):
     if pooling_mode not in POOLING_MODES:
         raise NotImplementedError("POOLING_MODE %r: expected one of %s" % (pooling_mode, ", ".join(POOLING_MODES)))
     if pooling_mode == "crop":
+        # crop_and_resize to P x P (or 2P x 2P before the 2x2 max pool) divides by P - 1: frcnn_crop_pool takes 2 <= P <= 16
+        if type(pooling_size) is not int or not 2 <= pooling_size <= N.ROI_MAX_POOLED:
+            raise ValueError("POOLING_SIZE must be an int in [2, %d] in 'crop' mode, got %r" % (N.ROI_MAX_POOLED, pooling_size))
         return None
     if type(pooling_size) is not int or not 1 <= pooling_size <= N.ROI_MAX_POOLED:
         raise ValueError("POOLING_SIZE must be an int in [1, %d] in %r mode, got %r" % (N.ROI_MAX_POOLED, pooling_mode, pooling_size))
@@ -768,6 +771,12 @@ def roi_align_option(pooling_mode, pooling_size, node):
     if type(aligned) is not bool:
         raise ValueError("ROI_ALIGN.ALIGNED must be a bool, got %r" % (aligned,))
     return (sr, aligned)
+
+
+def check_rpn_channels(n):
+    """cfg.RPN_CHANNELS: the fused RPN heads take it as K, which the conv kernel walks in 32-channel k-blocks."""
+    if not _is_int(n) or n <= 0 or n % 32:
+        raise ValueError("RPN_CHANNELS must be a positive multiple of 32, got %r" % (n,))
 
 
 def check_pool_boxes(pooling_mode, boxes, im_scales, blob_hw):

@@ -48,6 +48,7 @@ class Network(object):
         self.anchor_key = "%s|%s" % (self._anchor_scales, self._anchor_ratios)
         # POOLING_MODE 'crop' (the reference's), 'align' (RoIAlign, with cfg.ROI_ALIGN) or 'pool' (RoIPool); read at plan build
         roi_align = engine.roi_align_option(cfg.POOLING_MODE, cfg.POOLING_SIZE, cfg.ROI_ALIGN)
+        engine.check_rpn_channels(cfg.RPN_CHANNELS)
         self.options = dict(
             pooling_mode=cfg.POOLING_MODE, roi_align=roi_align,
             test_mode=cfg.TEST.MODE, use_e2e_tf=bool(cfg.USE_E2E_TF), use_gpu_nms=bool(cfg.USE_GPU_NMS),
@@ -110,7 +111,7 @@ class Network(object):
         (class count, anchor set, backbone).  Needs create_architecture() first.  -> list of messages."""
         from tf_faster_rcnn_b200 import synth
         return synth.check(self.arch_name(), tensors, self._num_classes, self._num_anchors,
-                           rpn_channels=int(cfg.RPN_CHANNELS),
+                           rpn_channels=int(cfg.RPN_CHANNELS), pooling_size=int(cfg.POOLING_SIZE),
                            depth_multiplier=float(getattr(self, "_depth_multiplier", 1.0)))
 
     def load_weights(self, tensors, strict=False):

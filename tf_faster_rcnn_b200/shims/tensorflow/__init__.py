@@ -39,7 +39,10 @@ class Session(object):
             from tf_faster_rcnn_b200 import synth
             for net in _networks():
                 if net.weights is None:
-                    net.load_weights(synth.make(net.arch_name(), net.num_classes, net.num_anchors))
+                    net.load_weights(synth.make(net.arch_name(), net.num_classes, net.num_anchors,
+                                                rpn_channels=int(net.options["rpn_channels"]),
+                                                pooling_size=int(net.options["pooling_size"]),
+                                                depth_multiplier=float(getattr(net, "_depth_multiplier", 1.0))))
             return None
         raise NotImplementedError("tensorflow shim: Session.run only supports the variable initializer; "
                                   "inference goes through Network.test_image / im_detect")

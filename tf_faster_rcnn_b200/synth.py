@@ -87,7 +87,7 @@ def resnet_block_plan(num_layers):
             ("block3", 256, [1] * n3), ("block4", 512, [1] * n4)]
 
 
-def make_vgg16(num_classes, num_anchors, seed=3, shapes_only=False, rpn_channels=512):
+def make_vgg16(num_classes, num_anchors, seed=3, shapes_only=False, rpn_channels=512, pooling_size=7):
     g = _Gen(seed, shapes_only)
     cin = 3
     for b, (n, c) in enumerate([(2, 64), (2, 128), (3, 256), (3, 512), (3, 512)], start=1):
@@ -96,7 +96,7 @@ def make_vgg16(num_classes, num_anchors, seed=3, shapes_only=False, rpn_channels
             g.conv("vgg_16/conv%d/conv%d_%d" % (b, b, i), 3, 3, cin, c, bias=True,
                    std=(np.sqrt(2.0 / 27) / 60.0 if cin == 3 else None))
             cin = c
-    g.fc("vgg_16/fc6", 7 * 7 * 512, 4096)
+    g.fc("vgg_16/fc6", pooling_size * pooling_size * 512, 4096)      # fc6 reads the flattened P x P x 512 pool5
     g.fc("vgg_16/fc7", 4096, 4096)
     g.heads("vgg_16", 512, 4096, num_classes, num_anchors, rpn_channels)
     return g.w
@@ -145,10 +145,11 @@ def make_mobilenet(num_classes, num_anchors, seed=3, mult=1.0, shapes_only=False
     return g.w
 
 
-def make(net, num_classes, num_anchors, seed=3, shapes_only=False, rpn_channels=512, depth_multiplier=1.0):
-    """net in {'vgg16','res50','res101','res152','mobile'} (tools/test_net.py:92-103 names)."""
+def make(net, num_classes, num_anchors, seed=3, shapes_only=False, rpn_channels=512, depth_multiplier=1.0, pooling_size=7):
+    """net in {'vgg16','res50','res101','res152','mobile'} (tools/test_net.py:92-103 names).  pooling_size (cfg.POOLING_SIZE)
+    sets VGG16's fc6 rows, P * P * 512; the other networks do not depend on it."""
     if net == "vgg16":
-        return make_vgg16(num_classes, num_anchors, seed, shapes_only, rpn_channels)
+        return make_vgg16(num_classes, num_anchors, seed, shapes_only, rpn_channels, pooling_size)
     if net.startswith("res"):
         return make_resnet(int(net[3:]), num_classes, num_anchors, seed, shapes_only, rpn_channels)
     if net == "mobile":
@@ -158,7 +159,7 @@ def make(net, num_classes, num_anchors, seed=3, shapes_only=False, rpn_channels=
 
 def spec(net, num_classes, num_anchors, **arch):
     """{TF variable name: shape} the TEST graph of `net` restores (the variables `make` draws), without drawing them.
-    arch: rpn_channels (cfg.RPN_CHANNELS), depth_multiplier (cfg.MOBILENET.DEPTH_MULTIPLIER)."""
+    arch: rpn_channels (cfg.RPN_CHANNELS), depth_multiplier (cfg.MOBILENET.DEPTH_MULTIPLIER), pooling_size (cfg.POOLING_SIZE)."""
     return make(net, num_classes, num_anchors, shapes_only=True, **arch)
 
 
