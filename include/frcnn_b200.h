@@ -387,6 +387,34 @@ int frcnn_detect_regions(const float* cls_prob_dev, const float* rois_dev, const
                          void* workspace_dev, size_t workspace_bytes, float* roi_box_dev, unsigned long long* key_dev,
                          float* boxes_out_dev, float* conf_out_dev, int* class_out_dev, int* index_out_dev, float* feat_out_dev,
                          int* count_out_dev, void* stream);
+/* Attribute head of the bottom-up regions (the Visual Genome model of Anderson et al. 2018: C = 1601 object classes, A = 401
+ * attribute classes with 0 = "no attribute"), an extension beyond the reference.  Per RoI, with F the fc7 width, E the embedding
+ * width and H the hidden width:
+ *   1. c = argmax of the RoI's class logits cls_score[i, 0..C) (background included), numpy's rule: the first NaN column if the
+ *      row holds one, else the first column holding the maximum;
+ *   2. e = cls_embedding[c] (a [C, E] table);
+ *   3. h = relu([fc7_i ; e] . W_fc_attr + b_fc_attr), fc7 first, W_fc_attr [F + E, H];
+ *   4. s = h . W_attr_score + b_attr_score (A logits), attr_prob = softmax(s);
+ *   5. attributes = 1 + argmax(attr_prob[1..A)) (the same argmax rule), attr_conf = attr_prob[attributes].
+ * It is computed on the M = min(max_boxes, r) region rows per image of frcnn_detect_regions (its index_out_dev / count_out_dev).
+ * Rows k >= count[b] are padding: emb zeros, attr_prob 0, attributes -1, attr_conf 0.  Steps 3 and 4 are two frcnn_conv_plan
+ * FCs (step 3 with the embedding as the second A source, in2_dev); the two entries below are steps 1-2 and the softmax plus
+ * step 5.  Both check their arguments before any CUDA call (FRCNN_ERR_ARG), allocate nothing and are capturable into a CUDA
+ * graph.
+ *
+ * Steps 1-2: cls_score_dev [batch*r, C] (frcnn_cls_finish's logits); index_dev / count_dev int32 [batch, M] / [batch] (region k
+ * of image b is RoI index[b, k] of that image; a row k < count whose index lies outside [0, r) is written as zeros);
+ * embedding_dev [C, embed_dim] -> emb_out_dev [batch*M, embed_dim], row b*M + k = embedding row c of that RoI.  Requirements:
+ * 2 <= C <= 4096, 1 <= M <= r, batch >= 1, embed_dim a positive multiple of 4, embedding_dev and emb_out_dev 16-byte aligned. */
+int frcnn_regions_attr_embed(const float* cls_score_dev, int r, int batch, int num_classes, const int* index_dev, const int* count_dev,
+                             int max_regions, const float* embedding_dev, int embed_dim, float* emb_out_dev, void* stream);
+/* Steps 4 (softmax) and 5: score_dev [batch*M, ld] attribute logits (columns A .. ld-1 are not read); per row, with
+ * frcnn_cls_finish's arithmetic: m = max of the A logits (fmaxf), e_j = expf(fl(s_j - m)), S = their sum (lane j mod 32 adds its
+ * columns in ascending order from +0, then 5 xor-shuffle adds), attr_prob_j = fl(e_j / S).  attributes_dev int32 [batch*M] and
+ * attr_conf_dev [batch*M] by step 5 on these fp32 probabilities; attr_prob_dev [batch*M, A].  Requirements: 2 <= A <= 4096,
+ * ld >= A, batch >= 1, M >= 1, every buffer 4-byte aligned. */
+int frcnn_attr_finish(const float* score_dev, int ld, int batch, int max_regions, int num_attributes, const int* count_dev,
+                      float* attr_prob_dev, int* attributes_dev, float* attr_conf_dev, void* stream);
 /* caller boxes -> RoI rows (the Fast R-CNN mode: TEST.HAS_RPN = False).  boxes_dev [batch, cap, 4] fp32 (x1,y1,x2,y2) in
  * ORIGINAL-image pixels; counts_dev int32 [batch]; im_meta_dev [batch, 3] as for frcnn_bbox_decode.  rois_dev [batch*cap, 5] =
  * (b, x1*s, y1*s, x2*s, y2*s), one fp32 multiply by im_meta's scale per coordinate, zeros past the count; num_rois_dev int32

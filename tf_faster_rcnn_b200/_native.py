@@ -78,6 +78,8 @@ SIGNATURES = {
     "frcnn_detect_features": (ci, [vp, vp, vp, ci, ci, ci, ci, ci, vp, vp, vp]),
     "frcnn_detect_regions": (ci, [vp, vp, vp, vp, vp, ci, ci, ci, ci, cf, cu, cf, ci, ci, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp, vp, vp,
                                   vp, vp]),
+    "frcnn_regions_attr_embed": (ci, [vp, ci, ci, ci, vp, vp, ci, vp, ci, vp, vp]),
+    "frcnn_attr_finish": (ci, [vp, ci, ci, ci, ci, vp, vp, vp, vp, vp]),
     "frcnn_boxes_to_rois": (ci, [vp, vp, vp, ci, ci, vp, vp, vp]),
     "frcnn_preprocess_hflip": (ci, [vp, ci, ci, C.POINTER(C.c_double), C.c_double, C.c_double, vp, ci, ci, vp]),
     "frcnn_aug_union": (ci, [C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), ip, ip, ci, ci, ci, vp, vp, vp, vp, vp]),

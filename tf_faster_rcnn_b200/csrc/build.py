@@ -11,7 +11,7 @@ from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 PKG = os.path.dirname(HERE)
-SOURCES = ["api.cu", "conv_gemm.cu", "simt_ops.cu", "nms.cu", "sort.cu"]
+SOURCES = ["api.cu", "conv_gemm.cu", "simt_ops.cu", "nms.cu", "sort.cu", "attributes.cu"]
 HEADERS = ["common.cuh", os.path.join("..", "..", "include", "frcnn_b200.h")]
 LIB = os.path.join(PKG, "libfrcnn_b200.so")
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a",

@@ -235,6 +235,7 @@ PostKey = collections.namedtuple("PostKey", "score_thresh nms_thresh use_gpu_nms
 # the options the bottom-up regions step is built for (PostStage._ensure_regions); conf_thresh is the fp32 threshold of region_args
 RegionKey = collections.namedtuple("RegionKey", "conf_thresh min_boxes max_boxes nms_thresh use_gpu_nms")
 REGION_FIELDS = ("boxes", "features", "conf", "classes", "roi_index")
+ATTR_FIELDS = ("attr_prob", "attributes", "attr_conf")     # the attribute head's region fields (options['attributes'] on)
 
 
 class PostStage:
@@ -251,6 +252,7 @@ class PostStage:
         self.post_key = None
         self.regions_key = self.regions_step = None                 # region mode (_ensure_regions)
         self.reg_box = self.reg_key = self.reg_out = self.reg_ws = None
+        self.attr_steps, self.attr_bufs = [], None                  # the attribute head on the regions (_build_attributes)
         self.recs = [None, None]
         self.rec = self.ndet = None    # views of the buffer the LAST detect launch wrote
         self.post_steps = [None, None]
@@ -329,6 +331,7 @@ class PostStage:
             self.reg_out = dict(boxes=ops.zeros((B, M, 4)), features=ops.zeros((B, M, fdim)), conf=ops.zeros((B, M)),
                                 classes=ops.zeros((B, M), dtype=torch.int32), roi_index=ops.zeros((B, M), dtype=torch.int32),
                                 count=ops.zeros((B,), dtype=torch.int32))
+            self._build_attributes(M)
         thr, flags = nms_threshold(key.nms_thresh, key.use_gpu_nms)
         out = self.reg_out
         keep = (self.keep, self.keep_cnt, self.keep_score) if per_class else (None, None, None)
@@ -339,12 +342,44 @@ class PostStage:
             del self.graphs[g]
         self.regions_key = key
 
+    def _build_attributes(self, M):
+        """The attribute head on reg_out's M rows per image when options['attributes'] = (A, E, H) is on (include/frcnn_b200.h,
+        frcnn_regions_attr_embed): its outputs join reg_out (attr_prob [B, M, A], attributes int32 [B, M], attr_conf [B, M]),
+        and its scratch is emb [B*M, E], hidden [B*M, H] and score [B*M, ld] (A zero-padded to a multiple of 4 columns, as the
+        cls|bbox head).  fc_attr reads the region features and emb as its two A sources, so the conv plans hold these buffers'
+        addresses and are rebuilt with them whenever M changes."""
+        attrs = self.net.options.get("attributes")
+        if attrs is None:
+            self.attr_steps, self.attr_bufs = [], None
+            return
+        A, E, H = attrs
+        wts, sc, B, C = self.net.weights, self.net.scope, self.batch, self.net.num_classes
+        rows, lda = B * M, (A + 3) // 4 * 4
+        out = self.reg_out
+        out["attr_prob"] = ops.zeros((B, M, A)); out["attributes"] = ops.zeros((B, M), dtype=torch.int32); out["attr_conf"] = ops.zeros((B, M))
+        emb, hidden, score = ops.zeros((rows, E)), ops.zeros((rows, H)), ops.zeros((rows, lda))
+        table = wts.dev(sc + "/cls_embedding", lambda: wts[sc + "/cls_embedding/weights"])
+
+        def padded_score():
+            w = np.zeros((1, 1, H, lda), F); b = np.zeros(lda, F)
+            w[0, 0, :, :A] = wts[sc + "/attr_score/weights"]; b[:A] = wts[sc + "/attr_score/biases"]
+            return w, None, b
+        fc_attr = ops.ConvPlan(out["features"].view(1, 1, rows, -1), wts.packed_conv(sc + "/fc_attr"), hidden.view(1, 1, rows, H),
+                               act=N.ACT_RELU, x2=emb.view(1, 1, rows, E))
+        attr_score = ops.ConvPlan(hidden.view(1, 1, rows, H), wts.packed_custom(sc + "/attr_score", padded_score), score.view(1, 1, rows, lda))
+        self.attr_bufs = dict(emb=emb, hidden=hidden, score=score, plans=(fc_attr, attr_score))
+        self.attr_steps = [lambda: ops.regions_attr_embed(self.cls_score, C, out["roi_index"], out["count"], table, emb),
+                           fc_attr.run, attr_score.run,
+                           lambda: ops.attr_finish(score, A, out["count"], out["attr_prob"], out["attributes"], out["attr_conf"])]
+
     def regions(self):
         """Host copy of the bottom-up regions of the batch after a 'regions' launch: per image a dict of boxes [n,4] fp32,
-        features [n,F] fp32, conf [n] fp32, classes [n] int32, roi_index [n] int32."""
+        features [n,F] fp32, conf [n] fp32, classes [n] int32, roi_index [n] int32, and with the attribute head attr_prob [n,A]
+        fp32, attributes [n] int32, attr_conf [n] fp32."""
         host = {k: v.cpu() for k, v in self.reg_out.items()}
         counts = host["count"].numpy()
-        return [{k: host[k][b, :int(counts[b])].numpy().copy() for k in REGION_FIELDS} for b in range(self.batch)]
+        fields = REGION_FIELDS + (ATTR_FIELDS if self.attr_bufs is not None else ())
+        return [{k: host[k][b, :int(counts[b])].numpy().copy() for k in fields} for b in range(self.batch)]
 
     def _select(self, slot):
         self.slot = slot
@@ -539,14 +574,16 @@ class ShapePlan(PostStage):
         self.feat_out = self.roi_out = self.features_step = None
         self.regions_key = self.regions_step = None
         self.reg_box = self.reg_key = self.reg_out = self.reg_ws = None
+        self.attr_steps, self.attr_bufs = [], None
 
     def steps_for(self, mode):
         """mode: 'test_image' (network outputs), 'im_detect' (+ decoded boxes), 'detect' (+ per-class NMS, cap, records),
         'features' (+ the head feature and RoI index of every record row); the last two after _begin_post.  'regions': the
-        network outputs + the bottom-up regions step (no box decode, no records), after _ensure_regions."""
+        network outputs + the bottom-up regions step (no box decode, no records) + the attribute head when it is on, after
+        _ensure_regions."""
         if mode in ("test_image", "regions"):
             fns = [fn for _, fn in self.tape.steps[:self.n_test_image_steps]]
-            return fns + [self.regions_step] if mode == "regions" else fns
+            return fns + [self.regions_step] + self.attr_steps if mode == "regions" else fns
         fns = [fn for _, fn in self.tape.steps[:self.n_im_detect_steps]]
         if mode in ("detect", "features"):
             fns.append(self.post_steps[self.slot])
@@ -777,6 +814,19 @@ def check_rpn_channels(n):
     """cfg.RPN_CHANNELS: the fused RPN heads take it as K, which the conv kernel walks in 32-channel k-blocks."""
     if not _is_int(n) or n <= 0 or n % 32:
         raise ValueError("RPN_CHANNELS must be a positive multiple of 32, got %r" % (n,))
+
+
+def attributes_option(node):
+    """cfg.ATTRIBUTES -> the network option: None when NUM_CLASSES is 0, else (NUM_CLASSES, EMBED_DIM, HIDDEN); ValueError before
+    any device work.  EMBED_DIM and HIDDEN are K of the fc_attr / attr_score FCs (EMBED_DIM as the second source's channels),
+    which the conv kernel walks in 32-channel k-blocks."""
+    a, e, h = node["NUM_CLASSES"], node["EMBED_DIM"], node["HIDDEN"]
+    if not _is_int(a) or not (a == 0 or 2 <= a <= MAX_CLASSES):
+        raise ValueError("ATTRIBUTES.NUM_CLASSES must be an integer, 0 (no attribute head) or in [2, %d], got %r" % (MAX_CLASSES, a))
+    for key, v in (("EMBED_DIM", e), ("HIDDEN", h)):
+        if not _is_int(v) or v <= 0 or v % 32:
+            raise ValueError("ATTRIBUTES.%s must be a positive multiple of 32, got %r" % (key, v))
+    return None if a == 0 else (int(a), int(e), int(h))
 
 
 def check_pool_boxes(pooling_mode, boxes, im_scales, blob_hw):

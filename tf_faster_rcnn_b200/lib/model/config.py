@@ -85,6 +85,10 @@ cfg = AttrDict(
     ANCHOR_SCALES=[8, 16, 32],
     ANCHOR_RATIOS=[0.5, 1, 2],
     RPN_CHANNELS=512,
+    # extension (the Visual Genome model of bottom-up-attention): the attribute head on detect_regions' regions.  NUM_CLASSES 0 =
+    # no head, else 2..4096 attribute classes (Visual Genome: 401, 0 = "no attribute"); EMBED_DIM (the class embedding) and HIDDEN
+    # (fc_attr's width) are positive multiples of 32
+    ATTRIBUTES=dict(NUM_CLASSES=0, EMBED_DIM=256, HIDDEN=512),
 )
 
 

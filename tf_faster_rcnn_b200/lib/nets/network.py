@@ -49,6 +49,7 @@ class Network(object):
         # POOLING_MODE 'crop' (the reference's), 'align' (RoIAlign, with cfg.ROI_ALIGN) or 'pool' (RoIPool); read at plan build
         roi_align = engine.roi_align_option(cfg.POOLING_MODE, cfg.POOLING_SIZE, cfg.ROI_ALIGN)
         engine.check_rpn_channels(cfg.RPN_CHANNELS)
+        attributes = engine.attributes_option(cfg.ATTRIBUTES)
         self.options = dict(
             pooling_mode=cfg.POOLING_MODE, roi_align=roi_align,
             test_mode=cfg.TEST.MODE, use_e2e_tf=bool(cfg.USE_E2E_TF), use_gpu_nms=bool(cfg.USE_GPU_NMS),
@@ -58,6 +59,7 @@ class Network(object):
             bbox_stds=tuple(cfg.TRAIN.BBOX_NORMALIZE_STDS), bbox_means=tuple(cfg.TRAIN.BBOX_NORMALIZE_MEANS),
             nms_thresh=cfg.TEST.NMS, max_per_image=100, score_thresh=0.0, rpn_channels=cfg.RPN_CHANNELS,
             soft_nms=engine.soft_nms_option(cfg.TEST.SOFT_NMS), box_vote=engine.box_vote_option(cfg.TEST.BBOX_VOTE),
+            attributes=attributes,
         )
         if self.options["test_mode"] not in ("nms", "top"):
             raise NotImplementedError
@@ -112,7 +114,7 @@ class Network(object):
         from tf_faster_rcnn_b200 import synth
         return synth.check(self.arch_name(), tensors, self._num_classes, self._num_anchors,
                            rpn_channels=int(cfg.RPN_CHANNELS), pooling_size=int(cfg.POOLING_SIZE),
-                           depth_multiplier=float(getattr(self, "_depth_multiplier", 1.0)))
+                           depth_multiplier=float(getattr(self, "_depth_multiplier", 1.0)), attributes=self.options["attributes"])
 
     def load_weights(self, tensors, strict=False):
         """tensors: dict TF-variable-name -> numpy array (HWIO convs, [in,out] FCs, BatchNorm stats).
@@ -238,7 +240,9 @@ class Network(object):
         min(max(count, min_boxes), max_boxes) by confidence.  One graph replay after the network outputs; the definition is
         frcnn_detect_regions' (include/frcnn_b200.h).  TEST.SOFT_NMS, TEST.BBOX_VOTE and max_per_image do not apply.
         -> (list over images of dict(boxes [n,4] fp32 unregressed RoI boxes in image pixels, features [n,F] fp32, conf [n] fp32,
-        classes [n] int32, roi_index [n] int32), plan).  ValueError before any device work for a conf_thresh outside [0, 1], counts
+        classes [n] int32, roi_index [n] int32), plan).  With the attribute head on (cfg.ATTRIBUTES.NUM_CLASSES = A > 0) each dict
+        also holds attr_prob [n, A] fp32, attributes [n] int32 (1 + the argmax of attr_prob[:, 1:]) and attr_conf [n] fp32, computed
+        on the device in the same replay (frcnn_regions_attr_embed / frcnn_attr_finish).  ValueError before any device work for a conf_thresh outside [0, 1], counts
         that are not integers with 0 <= min_boxes <= max_boxes, max_boxes >= 1, and with TEST.BBOX_AUG enabled."""
         _no_bbox_aug("bottom-up regions (detect_regions)")
         args = engine.region_args(conf_thresh, min_boxes, max_boxes)

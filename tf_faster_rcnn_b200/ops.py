@@ -360,6 +360,24 @@ def detect_regions(cls_prob, rois, num_rois, im_meta, fc7, num_classes, nms_thre
                                          _p(out["roi_index"]), _p(_f32(out["features"])), _p(out["count"]), _stream()), "detect_regions")
 
 
+def regions_attr_embed(cls_score, num_classes, index, count, embedding, emb_out):
+    """Attribute head steps 1-2 (frcnn_regions_attr_embed): cls_score [batch*r, C] logits, index / count int32 [batch, M] / [batch]
+    of detect_regions, embedding [C, E] -> emb_out [batch*M, E] = the embedding row of each region's argmax class (zeros past the
+    count)."""
+    batch, M = index.shape
+    r = cls_score.shape[0] // batch
+    N.check(N.lib().frcnn_regions_attr_embed(_p(_f32(cls_score)), r, batch, num_classes, _p(index), _p(count), M, _p(_f32(embedding)),
+                                             embedding.shape[1], _p(_f32(emb_out)), _stream()), "regions_attr_embed")
+
+
+def attr_finish(score, num_attributes, count, attr_prob, attributes, attr_conf):
+    """Attribute head softmax and step 5 (frcnn_attr_finish): score [batch*M, ld] logits, count int32 [batch] -> attr_prob
+    [batch, M, A], attributes int32 [batch, M] (-1 past the count), attr_conf [batch, M]."""
+    batch, M, _ = attr_prob.shape
+    N.check(N.lib().frcnn_attr_finish(_p(_f32(score)), score.shape[1], batch, M, num_attributes, _p(count), _p(_f32(attr_prob)),
+                                      _p(attributes), _p(_f32(attr_conf)), _stream()), "attr_finish")
+
+
 def boxes_to_rois(boxes, counts, im_meta, rois, num_rois):
     """boxes [batch, cap, 4] original-image pixels, counts int32 [batch], im_meta [batch, 3] -> rois [batch*cap, 5], num_rois."""
     batch, cap, _ = boxes.shape

@@ -42,7 +42,8 @@ class Session(object):
                     net.load_weights(synth.make(net.arch_name(), net.num_classes, net.num_anchors,
                                                 rpn_channels=int(net.options["rpn_channels"]),
                                                 pooling_size=int(net.options["pooling_size"]),
-                                                depth_multiplier=float(getattr(net, "_depth_multiplier", 1.0))))
+                                                depth_multiplier=float(getattr(net, "_depth_multiplier", 1.0)),
+                                                attributes=net.options["attributes"]))
             return None
         raise NotImplementedError("tensorflow shim: Session.run only supports the variable initializer; "
                                   "inference goes through Network.test_image / im_detect")

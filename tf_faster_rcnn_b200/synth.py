@@ -67,13 +67,25 @@ class _Gen:
         self.w[name + "/weights"] = (r.standard_normal((cin, cout)) * s).astype(F)
         self.w[name + "/biases"] = (r.standard_normal(cout) * bias_std).astype(F)
 
-    def heads(self, scope, c_body, c_tail, num_classes, num_anchors, rpn_channels=512):
-        """lib/nets/network.py:323-378: rpn_conv/3x3 (bias+ReLU, no BN), two 1x1 RPN heads, two FCs."""
+    def heads(self, scope, c_body, c_tail, num_classes, num_anchors, rpn_channels=512, attributes=None):
+        """lib/nets/network.py:323-378: rpn_conv/3x3 (bias+ReLU, no BN), two 1x1 RPN heads, two FCs; with attributes = (A, E, H)
+        also the attribute head: cls_embedding [C, E], fc_attr [c_tail + E, H], attr_score [H, A]."""
         self.conv(scope + "/rpn_conv/3x3", 3, 3, c_body, rpn_channels, bias=True)
         self.conv(scope + "/rpn_cls_score", 1, 1, rpn_channels, 2 * num_anchors, std=0.05, bias=True, bias_std=0.5)
         self.conv(scope + "/rpn_bbox_pred", 1, 1, rpn_channels, 4 * num_anchors, std=0.01, bias=True)
         self.fc(scope + "/cls_score", c_tail, num_classes, std=0.02, bias_std=0.5)
         self.fc(scope + "/bbox_pred", c_tail, 4 * num_classes, std=0.01)
+        if attributes is not None:
+            a, e, h = attributes
+            self.embedding(scope + "/cls_embedding", num_classes, e)
+            self.fc(scope + "/fc_attr", c_tail + e, h)
+            self.fc(scope + "/attr_score", h, a, std=0.05, bias_std=0.5)
+
+    def embedding(self, name, n, dim):
+        if self.shapes_only:
+            self.w[name + "/weights"] = (n, dim)
+            return
+        self.w[name + "/weights"] = (_rng(self.seed, name).standard_normal((n, dim)) * 0.5).astype(F)
 
 
 RESNET_UNITS = {50: (3, 4, 6, 3), 101: (3, 4, 23, 3), 152: (3, 8, 36, 3)}
@@ -87,7 +99,7 @@ def resnet_block_plan(num_layers):
             ("block3", 256, [1] * n3), ("block4", 512, [1] * n4)]
 
 
-def make_vgg16(num_classes, num_anchors, seed=3, shapes_only=False, rpn_channels=512, pooling_size=7):
+def make_vgg16(num_classes, num_anchors, seed=3, shapes_only=False, rpn_channels=512, pooling_size=7, attributes=None):
     g = _Gen(seed, shapes_only)
     cin = 3
     for b, (n, c) in enumerate([(2, 64), (2, 128), (3, 256), (3, 512), (3, 512)], start=1):
@@ -98,11 +110,11 @@ def make_vgg16(num_classes, num_anchors, seed=3, shapes_only=False, rpn_channels
             cin = c
     g.fc("vgg_16/fc6", pooling_size * pooling_size * 512, 4096)      # fc6 reads the flattened P x P x 512 pool5
     g.fc("vgg_16/fc7", 4096, 4096)
-    g.heads("vgg_16", 512, 4096, num_classes, num_anchors, rpn_channels)
+    g.heads("vgg_16", 512, 4096, num_classes, num_anchors, rpn_channels, attributes)
     return g.w
 
 
-def make_resnet(num_layers, num_classes, num_anchors, seed=3, shapes_only=False, rpn_channels=512):
+def make_resnet(num_layers, num_classes, num_anchors, seed=3, shapes_only=False, rpn_channels=512, attributes=None):
     g = _Gen(seed, shapes_only)
     sc = "resnet_v1_%d" % num_layers
     g.conv(sc + "/conv1", 7, 7, 3, 64, std=np.sqrt(2.0 / 147) / 60.0); g.bn(sc + "/conv1", 64)
@@ -116,7 +128,7 @@ def make_resnet(num_layers, num_classes, num_anchors, seed=3, shapes_only=False,
             g.conv(p + "/conv2", 3, 3, base, base); g.bn(p + "/conv2", base)
             g.conv(p + "/conv3", 1, 1, base, base * 4); g.bn(p + "/conv3", base * 4, gamma=(0.1, 0.3))
             cin = base * 4
-    g.heads(sc, 1024, 2048, num_classes, num_anchors, rpn_channels)
+    g.heads(sc, 1024, 2048, num_classes, num_anchors, rpn_channels, attributes)
     return g.w
 
 
@@ -129,7 +141,7 @@ def mobilenet_depth(d, mult=1.0, min_depth=8):
     return max(int(d * mult), min_depth)
 
 
-def make_mobilenet(num_classes, num_anchors, seed=3, mult=1.0, shapes_only=False, rpn_channels=512):
+def make_mobilenet(num_classes, num_anchors, seed=3, mult=1.0, shapes_only=False, rpn_channels=512, attributes=None):
     g = _Gen(seed, shapes_only)
     sc = "MobilenetV1"
     cin = 3
@@ -141,25 +153,28 @@ def make_mobilenet(num_classes, num_anchors, seed=3, mult=1.0, shapes_only=False
             g.dw("%s/Conv2d_%d_depthwise" % (sc, i), 3, cin); g.bn("%s/Conv2d_%d_depthwise" % (sc, i), cin)
             g.conv("%s/Conv2d_%d_pointwise" % (sc, i), 1, 1, cin, c); g.bn("%s/Conv2d_%d_pointwise" % (sc, i), c)
         cin = c
-    g.heads(sc, mobilenet_depth(512, mult), mobilenet_depth(1024, mult), num_classes, num_anchors, rpn_channels)
+    g.heads(sc, mobilenet_depth(512, mult), mobilenet_depth(1024, mult), num_classes, num_anchors, rpn_channels, attributes)
     return g.w
 
 
-def make(net, num_classes, num_anchors, seed=3, shapes_only=False, rpn_channels=512, depth_multiplier=1.0, pooling_size=7):
+def make(net, num_classes, num_anchors, seed=3, shapes_only=False, rpn_channels=512, depth_multiplier=1.0, pooling_size=7,
+         attributes=None):
     """net in {'vgg16','res50','res101','res152','mobile'} (tools/test_net.py:92-103 names).  pooling_size (cfg.POOLING_SIZE)
-    sets VGG16's fc6 rows, P * P * 512; the other networks do not depend on it."""
+    sets VGG16's fc6 rows, P * P * 512; the other networks do not depend on it.  attributes: None (no attribute head), or
+    (A, E, H) of cfg.ATTRIBUTES for the attribute head's variables; the other variables are the same either way."""
     if net == "vgg16":
-        return make_vgg16(num_classes, num_anchors, seed, shapes_only, rpn_channels, pooling_size)
+        return make_vgg16(num_classes, num_anchors, seed, shapes_only, rpn_channels, pooling_size, attributes)
     if net.startswith("res"):
-        return make_resnet(int(net[3:]), num_classes, num_anchors, seed, shapes_only, rpn_channels)
+        return make_resnet(int(net[3:]), num_classes, num_anchors, seed, shapes_only, rpn_channels, attributes)
     if net == "mobile":
-        return make_mobilenet(num_classes, num_anchors, seed, depth_multiplier, shapes_only, rpn_channels)
+        return make_mobilenet(num_classes, num_anchors, seed, depth_multiplier, shapes_only, rpn_channels, attributes)
     raise ValueError(net)
 
 
 def spec(net, num_classes, num_anchors, **arch):
     """{TF variable name: shape} the TEST graph of `net` restores (the variables `make` draws), without drawing them.
-    arch: rpn_channels (cfg.RPN_CHANNELS), depth_multiplier (cfg.MOBILENET.DEPTH_MULTIPLIER), pooling_size (cfg.POOLING_SIZE)."""
+    arch: rpn_channels (cfg.RPN_CHANNELS), depth_multiplier (cfg.MOBILENET.DEPTH_MULTIPLIER), pooling_size (cfg.POOLING_SIZE),
+    attributes (None, or (A, E, H): engine.attributes_option of cfg.ATTRIBUTES)."""
     return make(net, num_classes, num_anchors, shapes_only=True, **arch)
 
 

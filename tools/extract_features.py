@@ -16,6 +16,9 @@ their best class confidence after per-class NMS, 10-100 per image by default, wi
     boxes [n,4] fp32, features [n,F] fp32, conf [n] fp32, classes [n] int32, roi_index [n] int32, image_h, image_w, num_boxes;
 --tsv FILE also writes the protocol's TSV (image_id, image_w, image_h, num_boxes, boxes, features; the arrays as base64 of
 their float32 bytes), one row per image.  --regions and --boxes exclude each other.
+With the attribute head on (--set ATTRIBUTES.NUM_CLASSES 401), each --regions file also holds attr_prob [n,A] fp32, attributes
+[n] int32 and attr_conf [n] fp32, and the TSV gains the columns attrs_id (base64 of the int32 attributes) and attrs_conf
+(base64 of the float32 attr_conf) after the existing ones.
 Consecutive images whose blobs have the same shape are run together, up to --batch per device launch.  Without --model
 the network gets seeded synthetic weights."""
 import argparse
@@ -65,18 +68,26 @@ def image_boxes(boxes, imdb, i):
 
 
 TSV_FIELDS = ["image_id", "image_w", "image_h", "num_boxes", "boxes", "features"]
+TSV_ATTR_FIELDS = ["attrs_id", "attrs_conf"]       # appended with the attribute head on
 csv.field_size_limit(2 ** 31 - 1)
 
 
-def tsv_row(image_id, image_h, image_w, boxes, features):
-    """One row of the bottom-up-attention TSV: the arrays as base64 of their float32 bytes (row-major)."""
-    b64 = lambda a: base64.b64encode(np.ascontiguousarray(a, dtype=np.float32).tobytes()).decode("ascii")
-    return {"image_id": image_id, "image_w": int(image_w), "image_h": int(image_h), "num_boxes": int(boxes.shape[0]),
-            "boxes": b64(boxes), "features": b64(features)}
+def _b64(a, dtype=np.float32):
+    return base64.b64encode(np.ascontiguousarray(a, dtype=dtype).tobytes()).decode("ascii")
 
 
-def tsv_writer(f):
-    return csv.DictWriter(f, delimiter="\t", fieldnames=TSV_FIELDS)
+def tsv_row(image_id, image_h, image_w, boxes, features, attributes=None, attr_conf=None):
+    """One row of the bottom-up-attention TSV: the arrays as base64 of their float32 bytes (row-major); with the attribute head
+    also attrs_id (int32 bytes) and attrs_conf (float32 bytes)."""
+    row = {"image_id": image_id, "image_w": int(image_w), "image_h": int(image_h), "num_boxes": int(boxes.shape[0]),
+           "boxes": _b64(boxes), "features": _b64(features)}
+    if attributes is not None:
+        row.update(attrs_id=_b64(attributes, np.int32), attrs_conf=_b64(attr_conf))
+    return row
+
+
+def tsv_writer(f, attributes=False):
+    return csv.DictWriter(f, delimiter="\t", fieldnames=TSV_FIELDS + (TSV_ATTR_FIELDS if attributes else []))
 
 
 def extract(net, imdb, out_dir, batch=1, boxes=None, max_per_image=100, regions=None, tsv=None):
@@ -95,7 +106,8 @@ def extract(net, imdb, out_dir, batch=1, boxes=None, max_per_image=100, regions=
                 np.savez(os.path.join(out_dir, "%s.npz" % imdb.image_index[i]), image_h=hw[0], image_w=hw[1],
                          num_boxes=reg["boxes"].shape[0], **reg)
                 if tsv is not None:
-                    tsv.writerow(tsv_row(imdb.image_index[i], hw[0], hw[1], reg["boxes"], reg["features"]))
+                    tsv.writerow(tsv_row(imdb.image_index[i], hw[0], hw[1], reg["boxes"], reg["features"], reg.get("attributes"),
+                                         reg.get("attr_conf")))
         elif boxes is None:
             res, _ = net.detect_features(blobs, scales, hws)
             for (i, _, _, hw), (det, feats, roi) in zip(group, res):
@@ -138,7 +150,8 @@ def main(argv=None):
         raise SystemExit("--tsv needs --regions")
     if args.tsv:
         with open(args.tsv, "w", newline="") as f:
-            n = extract(net, imdb, args.out, max(1, args.batch), None, args.max_per_image, regions, tsv_writer(f))
+            n = extract(net, imdb, args.out, max(1, args.batch), None, args.max_per_image, regions,
+                        tsv_writer(f, net.options["attributes"] is not None))
     else:
         n = extract(net, imdb, args.out, max(1, args.batch), boxes, args.max_per_image, regions)
     print("wrote %d feature files to %s" % (n, args.out))

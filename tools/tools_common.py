@@ -12,5 +12,5 @@ def build_net(net_name, num_classes, model=None):
     if model:
         net.load_weights(checkpoint.load_variables(model), strict=True)   # TF V2 bundle or .npz
     else:
-        net.load_weights(synth.make(net_name, num_classes, net.num_anchors))
+        net.load_weights(synth.make(net_name, num_classes, net.num_anchors, attributes=net.options["attributes"]))
     return net
