@@ -30,9 +30,12 @@ def weight_exponent(w):
 
 
 def rna_tf32(x):
-    """fp32 -> tf32 (10 explicit mantissa bits), nearest, ties away from zero, on the bit pattern (finite inputs)."""
-    u = np.asarray(x, np.float32).view(np.uint32).astype(np.uint64)
-    return ((((u + (1 << 12)) >> 13) << 13).astype(np.uint32)).view(np.float32)
+    """fp32 -> tf32 (10 explicit mantissa bits), nearest, ties away from zero, on the bit pattern; a NaN stays a NaN (as
+    through cvt.rna: the bit arithmetic alone would carry a NaN with a full payload, such as 0x7fffffff, to -0.0)."""
+    x = np.asarray(x, np.float32)
+    u = x.view(np.uint32).astype(np.uint64)
+    r = ((((u + (1 << 12)) >> 13) << 13).astype(np.uint32)).view(np.float32)
+    return np.where(np.isnan(x), x, r)
 
 
 def rn_f16(x, saturate=False):
